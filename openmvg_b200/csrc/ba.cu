@@ -8,6 +8,7 @@
 // termination decisions from a handful of scalars read back once per LM iteration.
 #include "ba_kernels.cuh"
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 #include <cmath>
@@ -73,7 +74,8 @@ struct omvg_ba_ctx {
   DevBuf<int> fail;
   DevBuf<unsigned long long> pcg_tim;
   DevBuf<double> corner_rep;
-  DevBuf<double> GE;                        // per observation { Einv E'Fc, E'Fc } of the split Schur step
+  DevBuf<double> H;                         // per observation L^-1 E'Fc of the split Schur step
+  DevBuf<int2> pair; DevBuf<int> pair_start, chunk_blk, chunk_first, ticket; DevBuf<double> gpart; int n_chunks = 0;   // co-visibility lists (schur_gather_kernel)
   // optional extensions: GCP weights / flags / fixed landmarks, pose-centre priors
   DevBuf<double> obs_w; DevBuf<unsigned char> obs_flags, pt_fixed; DevBuf<unsigned> pt_mask;
   DevBuf<unsigned char> pt_gcp, pt_removed, pt_now; DevBuf<unsigned> rej_bits; DevBuf<unsigned long long> rej_cnt;   // outlier rejection (omvg_ba_reject_outliers)
@@ -256,6 +258,61 @@ int read_scalars(omvg_ba_ctx *c) {
 }
 double host_gmax(const omvg_ba_ctx *c) { double m = 0; for (int i = 0; i < 192; ++i) m = std::max(m, c->h_scal[S_COUNT + i]); return m; }
 
+// Co-visibility lists of schur_gather_kernel: the observation pairs of every upper / diagonal camera block in landmark
+// order (pair_count / pair_emit, stable radix sort by block), cut into chunks of at most GATHER_CHUNK pairs.
+// hp / hcols: BSR row pointers and columns on the host.  The sort's buffers (16 B per pair) live in the H records
+// (144 B per observation), which the first run overwrites; only when a scene has more than ~8 pairs per observation
+// (long tracks) do they take memory of their own.
+int build_pairs(omvg_ba_ctx *c, const std::vector<int> &hp, const std::vector<int> &hcols) {
+  cudaStream_t s = c->stream;
+  int rc;
+  const unsigned gp = (unsigned)((c->np + 255) / 256);
+  const Bsr B{c->bitmap.p, c->wprefix.p, c->rowptr.p, c->words};
+  long long total = 0;
+  DevBuf<long long> cnt, off; DevBuf<unsigned char> tmp, own;
+  if ((rc = c->H.alloc(HREC * (size_t)c->no)) || (rc = cnt.alloc(c->np + 1)) || (rc = off.alloc(c->np + 1))) return rc;
+  OMVG_CUDA(cudaMemsetAsync(cnt.p + c->np, 0, sizeof(long long), s));
+  pair_count_kernel<<<gp, 256, 0, s>>>(c->pt_start.p, c->pt_single.p, c->obs_pose.p, c->np, cnt.p); LAUNCH_CHECK();
+  { size_t tb = 0; OMVG_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt.p, off.p, c->np + 1, s));
+    if ((rc = tmp.alloc(tb))) return rc;
+    OMVG_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tb, cnt.p, off.p, c->np + 1, s)); }
+  OMVG_CUDA(cudaMemcpyAsync(&total, off.p + c->np, sizeof total, cudaMemcpyDeviceToHost, s));
+  OMVG_CUDA(cudaStreamSynchronize(s));
+  if (total > std::numeric_limits<int>::max()) return fail(OMVG_E_UNSUPPORTED, "%lld camera-block pairs: more than 2^31", total);
+  const int npair = (int)total;
+  if ((rc = c->pair.alloc(npair)) || (rc = c->pair_start.alloc(c->nnzb + 1))) return rc;
+  { int bits = 1; while ((1ll << bits) < c->nnzb) ++bits;
+    const size_t kb = ((size_t)npair * sizeof(int) + 255) & ~(size_t)255, vb = ((size_t)npair * sizeof(int2) + 255) & ~(size_t)255;
+    size_t tb = 0;
+    { cub::DoubleBuffer<int> keys(nullptr, nullptr); cub::DoubleBuffer<int2> vals(nullptr, nullptr);
+      OMVG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, keys, vals, npair, 0, bits, s)); }
+    unsigned char *sc = reinterpret_cast<unsigned char *>(c->H.p);
+    if (2 * kb + vb + tb > c->H.n * sizeof(double)) { if ((rc = own.alloc(2 * kb + vb + tb))) return rc; sc = own.p; }
+    int *k0 = reinterpret_cast<int *>(sc), *k1 = reinterpret_cast<int *>(sc + kb);
+    int2 *v1 = reinterpret_cast<int2 *>(sc + 2 * kb);
+    pair_emit_kernel<<<gp, 256, 0, s>>>(c->pt_start.p, c->pt_single.p, c->obs_pose.p, c->np, off.p, B, k0, c->pair.p); LAUNCH_CHECK();
+    cub::DoubleBuffer<int> keys(k0, k1); cub::DoubleBuffer<int2> vals(c->pair.p, v1);
+    OMVG_CUDA(cub::DeviceRadixSort::SortPairs(sc + 2 * kb + vb, tb, keys, vals, npair, 0, bits, s));
+    if (npair && vals.Current() != c->pair.p) OMVG_CUDA(cudaMemcpyAsync(c->pair.p, vals.Current(), (size_t)npair * sizeof(int2), cudaMemcpyDeviceToDevice, s));
+    setup_starts_kernel<<<(unsigned)((npair + 256) / 256), 256, 0, s>>>(keys.Current(), npair, c->nnzb, c->pair_start.p); LAUNCH_CHECK(); }
+  std::vector<int> ps(c->nnzb + 1), first(c->nnzb + 1, 0), blk;
+  OMVG_CUDA(cudaMemcpyAsync(ps.data(), c->pair_start.p, (c->nnzb + 1) * sizeof(int), cudaMemcpyDeviceToHost, s));
+  OMVG_CUDA(cudaStreamSynchronize(s));
+  for (int a = 0; a < c->nc; ++a)
+    for (int e = hp[a]; e < hp[a + 1]; ++e) {
+      first[e] = (int)blk.size();
+      if (hcols[e] < a) continue;                       // lower blocks are stored as transposes of their upper partner
+      blk.insert(blk.end(), std::max(1, (ps[e + 1] - ps[e] + GATHER_CHUNK - 1) / GATHER_CHUNK), e);
+    }
+  first[c->nnzb] = (int)blk.size(); c->n_chunks = (int)blk.size();
+  if ((rc = upload(c->chunk_blk, blk.data(), blk.size(), s)) || (rc = upload(c->chunk_first, first.data(), first.size(), s))) return rc;
+  if ((rc = c->ticket.alloc(c->nnzb)) || (rc = c->gpart.alloc(36 * (size_t)c->n_chunks))) return rc;
+  OMVG_CUDA(cudaMemsetAsync(c->ticket.p, 0, c->nnzb * sizeof(int), s));
+  OMVG_CUDA(cudaStreamSynchronize(s));
+  c->launches += 3;
+  return OMVG_OK;
+}
+
 int build_structure(omvg_ba_ctx *c) {
   c->words = (c->nc + 31) / 32;
   int rc;
@@ -370,7 +427,8 @@ int build_structure(omvg_ba_ctx *c) {
   if ((rc = c->cCv2.alloc((size_t)MAXRHS * nco_max + 1)) || (rc = c->cAW.alloc((size_t)MAXRHS * nco_max + 1))) return rc;
   if ((rc = c->bP2.alloc((size_t)MAXRHS * 6 * c->nc))) return rc;
   OMVG_CUDA(cudaStreamSynchronize(c->stream));
-  return c->Scc.alloc((size_t)c->nnzb * 36);
+  if ((rc = c->Scc.alloc((size_t)c->nnzb * 36))) return rc;
+  return build_pairs(c, hp, hcols);
 }
 
 }  // namespace
@@ -627,24 +685,25 @@ int omvg_ba_run(omvg_ba_ctx *c, const omvg_ba_options *O, omvg_ba_summary *sum) 
     // ---- reduced camera system
     const bool split_schur = m.pts_free && !getenv("OMVG_BA_SCHUR1") && !getenv("OMVG_BA_SCHUR2");
     if (split_schur && !c->corner_rep.p) { if ((rc = c->corner_rep.alloc((size_t)CORNER_REPS * (KI * KI + KI)))) return rc; }
-    { Zero4 Z{}; Z.p[0] = c->Scc.p; Z.n[0] = (long long)c->nnzb * 36; Z.p[1] = c->Sci.p; Z.n[1] = (long long)c->Sci.n; Z.p[2] = c->Sii.p; Z.n[2] = (long long)c->Sii.n;
-      Z.p[3] = split_schur ? c->corner_rep.p : c->rhs.p; Z.n[3] = split_schur ? (long long)c->corner_rep.n : 0;     // (rhs is fully written by s_init_kernel)
-      const int nb = (int)std::max<long long>(1, std::min<long long>(4 * c->n_sms, (Z.n[0] + 255) / 256));
+    // (the split path's schur_gather_kernel writes every block of Scc, rhs is fully written by s_init_kernel)
+    { Zero4 Z{}; Z.p[0] = c->Scc.p; Z.n[0] = split_schur ? 0 : (long long)c->nnzb * 36; Z.p[1] = c->Sci.p; Z.n[1] = (long long)c->Sci.n; Z.p[2] = c->Sii.p; Z.n[2] = (long long)c->Sii.n;
+      Z.p[3] = split_schur ? c->corner_rep.p : c->rhs.p; Z.n[3] = split_schur ? (long long)c->corner_rep.n : 0;
+      const int nb = (int)std::max<long long>(1, std::min<long long>(4 * c->n_sms, (std::max(Z.n[0], Z.n[1]) + 255) / 256));
       zero4_kernel<<<dim3(nb, 4), 256, 0, c->stream>>>(Z); LAUNCH_CHECK(); }
     SchurArgs SA{}; SA.r = c->r.p; SA.Jp = c->Jp.p; SA.Jc = c->Jc.p; SA.Ji = c->Ji.p; SA.EtE = c->EtE.p; SA.Etb = c->Etb.p; SA.EtFi = c->EtFi.p; SA.lmD_pt = c->lmD_pt.p; SA.pt_single = c->pt_single.p; SA.FtF = c->FtF.p; SA.FiFi = c->FiFi.p; SA.g_cam = c->g_cam.p; SA.g_intr = c->g_intr.p;
     SA.obs_pose = c->obs_pose.p; SA.obs_intr = c->obs_intr.p; SA.obs_pt = c->obs_pt.p; SA.pt_start = c->pt_start.p; SA.n = c->no; SA.n_poses = c->nc; SA.n_intr = c->ni;
     SA.pts_free = m.pts_free; SA.kiu = c->kiu; SA.bsr = Bsr{c->bitmap.p, c->wprefix.p, c->rowptr.p, c->words}; SA.Scc = c->Scc.p; SA.Sci = c->Sci.p; SA.Sii = c->Sii.p; SA.rhs = c->rhs.p;
     SA.Einv = c->Einv.p; SA.fail = c->fail.p;
-    { const int ninit = std::max(std::max(36 * c->nc, 64 * c->ni), c->nred); s_init_kernel<<<(ninit + 255) / 256, 256, 0, c->stream>>>(SA); LAUNCH_CHECK(); }
+    { SchurArgs SI = SA; if (split_schur) SI.Scc = nullptr;
+      const int ninit = std::max(std::max(36 * c->nc, 64 * c->ni), c->nred); s_init_kernel<<<(ninit + 255) / 256, 256, 0, c->stream>>>(SI); LAUNCH_CHECK(); }
     static const bool schur1 = getenv("OMVG_BA_SCHUR1") != nullptr;
     SA.n_points = c->np;
     static const bool schur2 = getenv("OMVG_BA_SCHUR2") != nullptr;      // fused warp-per-landmark kernel (A/B)
-    if (m.pts_free && !schur1 && !schur2) {
-      if (!c->GE.p) { if ((rc = c->GE.alloc(36 * (size_t)c->no))) return rc; }
+    if (split_schur) {
       { const unsigned sg = (unsigned)((c->no + SCHUR_THREADS - 1) / SCHUR_THREADS);
         static const bool minb4 = getenv("OMVG_BA_STAGE_MINB") && atoi(getenv("OMVG_BA_STAGE_MINB")) == 4;   // A/B: 128 registers, 4 CTAs per SM
-#define STAGE(K) do { if (minb4) schur_stage_kernel<K, 4><<<sg, SCHUR_THREADS, 0, c->stream>>>(SA, c->GE.p, c->corner_rep.p); \
-                      else schur_stage_kernel<K, 5><<<sg, SCHUR_THREADS, 0, c->stream>>>(SA, c->GE.p, c->corner_rep.p); } while (0)
+#define STAGE(K) do { if (minb4) schur_stage_kernel<K, 4><<<sg, SCHUR_THREADS, 0, c->stream>>>(SA, c->H.p, c->corner_rep.p); \
+                      else schur_stage_kernel<K, 5><<<sg, SCHUR_THREADS, 0, c->stream>>>(SA, c->H.p, c->corner_rep.p); } while (0)
         switch (c->kiu) {        // intrinsic columns in use (as for the column sums)
           case 3: STAGE(3); break;
           case 4: STAGE(4); break;
@@ -656,8 +715,8 @@ int omvg_ba_run(omvg_ba_ctx *c, const omvg_ba_options *O, omvg_ba_summary *sum) 
       }
       LAUNCH_CHECK();
       corner_fold_kernel<<<1, 96, 0, c->stream>>>(c->corner_rep.p, c->obs_intr.p, c->nc, c->ni, c->Sii.p, c->rhs.p); LAUNCH_CHECK(); c->launches++;
-      static const int occ2 = [] { int o = 1; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, schur_pair_kernel, 256, 0); return std::max(1, o); }();   // (thread-safe: Adjust may run on several host threads)
-      schur_pair_kernel<<<c->n_sms * occ2, 256, 0, c->stream>>>(SA, c->GE.p); LAUNCH_CHECK(); c->launches += 2;
+      GatherArgs G{c->H.p, c->FtF.p, c->pair.p, c->pair_start.p, c->chunk_blk.p, c->chunk_first.p, c->brow.p, c->cols.p, SA.bsr, c->Scc.p, c->gpart.p, c->ticket.p, c->n_chunks};
+      schur_gather_kernel<<<(c->n_chunks + 7) / 8, 256, 0, c->stream>>>(G); LAUNCH_CHECK(); c->launches += 2;
       SA.skip_fast = 1;
     } else
     if (m.pts_free && !schur1) {
@@ -668,8 +727,8 @@ int omvg_ba_run(omvg_ba_ctx *c, const omvg_ba_options *O, omvg_ba_summary *sum) 
       SA.skip_fast = 1;
     }
     if (!m.pts_free || schur1 || c->n_slow > 0) { schur_kernel<<<(unsigned)((c->no + SCHUR_THREADS - 1) / SCHUR_THREADS), SCHUR_THREADS, 0, c->stream>>>(SA); LAUNCH_CHECK(); }
-    mirror_kernel<<<(c->nc * 32 + 255) / 256, 256, 0, c->stream>>>(c->Scc.p, SA.bsr, c->cols.p, c->nc); LAUNCH_CHECK();
-    c->launches += 2;
+    if (!split_schur || c->n_slow > 0) { mirror_kernel<<<(c->nc * 32 + 255) / 256, 256, 0, c->stream>>>(c->Scc.p, SA.bsr, c->cols.p, c->nc); LAUNCH_CHECK(); c->launches++; }
+    c->launches++;
     finish_cam_kernel<<<(c->nc + 63) / 64, 64, 0, c->stream>>>(c->Scc.p, SA.bsr, c->lmD_cam.p, m.pose_mask, c->nc, c->Minv_c.p, c->fail.p, use_dense ? 0 : 1); LAUNCH_CHECK();
     finish_intr_kernel<<<1, 256, 0, c->stream>>>(c->Sii.p, c->lmD_intr.p, c->intr_mask.p, c->ni8, c->Minv_i.p, c->work_i.p, c->fail.p, (use_pcg2 || use_dense) ? 0 : 1); LAUNCH_CHECK();
     // ---- PCG on S z = rhs

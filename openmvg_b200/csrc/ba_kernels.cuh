@@ -53,6 +53,13 @@ template <int THREADS> __device__ __forceinline__ double block_sum(double v, dou
   return t;
 }
 
+// lower Cholesky factor of a 3x3 SPD matrix, both packed by rows: m = {a00,a10,a11,a20,a21,a22} -> L = {l00,l10,l11,l20,l21,l22}
+// (the same expressions as inv3_spd, which checks the pivots)
+__device__ __forceinline__ void chol3(const double m[6], double L[6]) {
+  L[0] = sqrt(m[0]); L[1] = m[1] / L[0]; L[3] = m[3] / L[0];
+  L[2] = sqrt(m[2] - L[1] * L[1]); L[4] = (m[4] - L[3] * L[1]) / L[2];
+  L[5] = sqrt(m[5] - L[3] * L[3] - L[4] * L[4]);
+}
 // 3x3 SPD inverse through LLT (invert_psd_matrix.h:56-59). m = {a00,a10,a11,a20,a21,a22}
 __device__ __forceinline__ bool inv3_spd(const double m[6], double inv[9]) {
   const double l00 = sqrt(m[0]), l10 = m[1] / l00, l20 = m[3] / l00;
@@ -675,10 +682,11 @@ struct SchurArgs {
 
 // Radius-independent part of the reduced system, computed once per Jacobian evaluation without atomics
 // (cam_colsum / intr_colsum): Scc(p,p) = Fc'Fc, Sii(q,q) = Fi'Fi, rhs = [Fc'r ; Fi'r].  S must be zeroed first.
+// With A.Scc null the camera blocks are left alone (schur_gather_kernel writes Scc(p,p) = Fc'Fc - sum itself).
 __global__ void s_init_kernel(SchurArgs A) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int nc36 = 36 * A.n_poses, ni64 = 64 * A.n_intr, nred = 6 * A.n_poses + KI * A.n_intr;
-  if (i < nc36) { const int p = i / 36; A.Scc[36 * (size_t)bsr_find(A.bsr, p, p) + i % 36] = A.FtF[i]; }
+  if (i < nc36 && A.Scc) { const int p = i / 36; A.Scc[36 * (size_t)bsr_find(A.bsr, p, p) + i % 36] = A.FtF[i]; }
   if (i < ni64) { const int q = i / 64, e = i % 64; A.Sii[(size_t)(KI * q + e / KI) * (KI * A.n_intr) + KI * q + e % KI] = A.FiFi[i]; }
   if (i < nred) A.rhs[i] = i < 6 * A.n_poses ? A.g_cam[i] : A.g_intr[i - 6 * A.n_poses];
 }
@@ -948,38 +956,46 @@ __global__ void __launch_bounds__(32 * SCHUR2_WARPS, MINB) schur_point_kernel(Sc
   }
 }
 
-// ---- split form of the warp-per-landmark Schur step (default): the staging half needs ~160 registers, the pair
-// walk ~40; in one kernel the walk ran at 12-20 warps per SM and was latency-bound (0.94 ms).  Here
-//   schur_stage_kernel : thread per observation (coalesced component-major loads), per-observation border / rhs
-//                        terms, writes GE[obs] = { Einv E'Fc (18), E'Fc (18) }  (288 B per observation)
-//   schur_pair_kernel  : warp per landmark, lane e adds element e of block (cam_t, cam_u) reading GE through L1
+// ---- split form of the warp-per-landmark Schur step (default).  With E'E + D^2 = L L' per landmark and
+// H_t = L^-1 E'Fc_t (3 x 6) per observation, a camera block is a plain sum  Scc(a,b) = [a == b] Fc'Fc - sum H_t' H_u
+// over the observation pairs (t, u) of one landmark with cam(t) = a, cam(u) = b.  The pairs of every block are listed
+// once per problem (pair_count / pair_emit, sorted by block in omvg_ba_create), so:
+//   schur_stage_kernel  : thread per observation (coalesced component-major loads), per-observation border / rhs
+//                         terms, writes H[obs] (144 B per observation, in observation order)
+//   schur_gather_kernel : warp per block (or per chunk of a long pair list), sums in registers in list order and
+//                         stores every element once: no atomics, and the same bits on every run (the landmarks
+//                         schur_kernel takes still add theirs with atomics)
 // KIU = intrinsic columns in use (3 pinhole .. 8 Brown): the generic 8-column body kept 16 Jacobian and 24 EtFi values
-// live per thread (162 registers, 3 CTAs per SM, 17 % of the warps active, 5x off its DRAM time).  The 36 doubles of an
-// observation's {E^-1 E'F, E'F} record go through shared memory so that a warp writes its 32 records (9 KB, contiguous)
-// with full 256-byte stores instead of 36 scattered 8-byte stores per lane.
-constexpr int GE_LD = 37;                            // padded record stride in shared memory (conflict-free for both phases)
+// live per thread (162 registers, 3 CTAs per SM, 17 % of the warps active, 5x off its DRAM time).  An observation's
+// {H, E'F} goes through shared memory so that a warp writes its 32 H records (4.5 KB, contiguous) with full 256-byte
+// stores instead of 18 scattered 8-byte stores per lane, and the border terms read E'F back from there.
+// (H in camera order, so that a block reads two compact regions, was measured on config 2 on an H100 SXM at 700 W: the
+// gather time did not change and the scattered record stores cost the stage kernel 0.12 ms per LM step.)
+constexpr int HREC = 18;                             // doubles per H record
+constexpr int STAGE_LD = 37;                         // padded record stride in shared memory (conflict-free for both phases)
 template <int KIU, int MINB>
-__global__ void __launch_bounds__(SCHUR_THREADS, MINB) schur_stage_kernel(SchurArgs A, double *__restrict__ GE, double *__restrict__ corner_rep) {
+__global__ void __launch_bounds__(SCHUR_THREADS, MINB) schur_stage_kernel(SchurArgs A, double *__restrict__ H, double *__restrict__ corner_rep) {
   // The intrinsics corner (and its rhs) of group q0 is hit once per landmark: accumulate into CORNER_REPS replicas
   // with native FP64 REDs (shared-memory double atomics are CAS loops: they cost 0.3 ms here) and fold them after.
-  __shared__ double ge_s[SCHUR_THREADS / 32][32 * GE_LD];
+  __shared__ double rec_s[SCHUR_THREADS / 32][32 * STAGE_LD];
   const long long t = (long long)blockIdx.x * SCHUR_THREADS + threadIdx.x;
   const long long n = A.n;
   const int nred_c = 6 * A.n_poses, ni8 = KI * A.n_intr;
   const int q0 = A.obs_intr[0];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   double *s_ii = corner_rep + (size_t)(blockIdx.x % CORNER_REPS) * (KI * KI + KI);
-  double *gs = ge_s[warp] + lane * GE_LD;
+  double *gs = rec_s[warp] + lane * STAGE_LD;
   bool mine = t < n;
   int j = 0;
   if (mine) { j = A.obs_pt[t]; const int K = A.pt_start[j + 1] - A.pt_start[j]; mine = A.pt_single[j] != 0 && K <= 32; }
   if (mine) {
     const int ct = A.obs_pose[t], qt = A.obs_intr[t];
-    double inv[9], ie[3], m[6];
+    double inv[9], ie[3], m[6], L[6];
     { const double *E = A.EtE + 6 * (size_t)j;
       const double d0 = A.lmD_pt[3 * j], d1 = A.lmD_pt[3 * j + 1], d2 = A.lmD_pt[3 * j + 2];
       m[0] = E[0] + d0 * d0; m[1] = E[1]; m[2] = E[2] + d1 * d1; m[3] = E[3]; m[4] = E[4]; m[5] = E[5] + d2 * d2; }
     if (!inv3_spd(m, inv)) atomicExch(A.fail, 1);
+    chol3(m, L);
     { const double *eb = A.Etb + 3 * (size_t)j;
       #pragma unroll
       for (int a = 0; a < 3; ++a) ie[a] = inv[a * 3] * eb[0] + inv[a * 3 + 1] * eb[1] + inv[a * 3 + 2] * eb[2]; }
@@ -990,20 +1006,20 @@ __global__ void __launch_bounds__(SCHUR_THREADS, MINB) schur_stage_kernel(SchurA
     for (int k = 0; k < 12; ++k) jc[k] = A.Jc[k * n + t];
     #pragma unroll
     for (int k = 0; k < 6; ++k) jp[k] = A.Jp[k * n + t];
-    // E'F (3 x 6) and E^-1 E'F: the record for the pair walk.  Staged in shared memory (written to GE below) and read
-    // back from there by the border terms, so that the 18 + 18 values are not live in registers next to jc / inv.
+    // E'F (3 x 6) and H = L^-1 E'F (forward substitution, column by column), staged in shared memory
     { double efc[18];
       #pragma unroll
       for (int a = 0; a < 3; ++a)
         #pragma unroll
         for (int c = 0; c < 6; ++c) efc[a * 6 + c] = jp[a] * jc[c] + jp[3 + a] * jc[6 + c];
+      const double r0 = 1.0 / L[0], r1 = 1.0 / L[2], r2 = 1.0 / L[5];
       #pragma unroll
-      for (int a = 0; a < 3; ++a)
-        #pragma unroll
-        for (int c = 0; c < 6; ++c) {
-          gs[a * 6 + c] = inv[a * 3] * efc[c] + inv[a * 3 + 1] * efc[6 + c] + inv[a * 3 + 2] * efc[12 + c];
-          gs[18 + a * 6 + c] = efc[a * 6 + c];
-        } }
+      for (int c = 0; c < 6; ++c) {
+        const double h0 = efc[c] * r0, h1 = (efc[6 + c] - L[1] * h0) * r1, h2 = (efc[12 + c] - L[3] * h0 - L[4] * h1) * r2;
+        gs[c] = h0; gs[6 + c] = h1; gs[12 + c] = h2;
+      }
+      #pragma unroll
+      for (int k = 0; k < 18; ++k) gs[18 + k] = efc[k]; }
     __syncwarp(__activemask());
     const double *ef = gs + 18;
     #pragma unroll
@@ -1032,16 +1048,16 @@ __global__ void __launch_bounds__(SCHUR_THREADS, MINB) schur_stage_kernel(SchurA
     }
   } else {
     #pragma unroll
-    for (int k = 0; k < 36; ++k) gs[k] = 0.0;         // (records of landmarks the general kernel handles are not read)
+    for (int k = 0; k < HREC; ++k) gs[k] = 0.0;       // (records of landmarks the general kernel handles are not read)
   }
   __syncwarp();
-  // the warp's 32 records are contiguous in GE: 36 coalesced 256-byte stores
+  // the warp's 32 records are contiguous in H: 18 coalesced 256-byte stores
   { const long long t0 = (long long)blockIdx.x * SCHUR_THREADS + 32 * warp;
     const long long nrec = n - t0 < 32 ? n - t0 : 32;
     if (nrec > 0) {
-      double *dst = GE + 36 * (size_t)t0;
-      #pragma unroll 4
-      for (int e = lane; e < 36 * (int)nrec; e += 32) dst[e] = ge_s[warp][(e / 36) * GE_LD + e % 36];
+      double *dst = H + HREC * (size_t)t0;
+      #pragma unroll 2
+      for (int e = lane; e < HREC * (int)nrec; e += 32) dst[e] = rec_s[warp][(e / HREC) * STAGE_LD + e % HREC];
     } }
 }
 // folds the corner replicas of schur_stage_kernel into Sii / rhs of group q0 (fixed order)
@@ -1053,46 +1069,113 @@ __global__ void corner_fold_kernel(const double *__restrict__ corner_rep, const 
   if (e < KI * KI) atomicAdd(&Sii[(size_t)(KI * q0 + e / KI) * ni8 + KI * q0 + e % KI], v);
   else atomicAdd(&rhs[6 * n_poses + KI * q0 + (e - KI * KI)], v);
 }
-__global__ void __launch_bounds__(256) schur_pair_kernel(SchurArgs A, const double *__restrict__ GE) {
-  const int lane = threadIdx.x & 31;
-  const int gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
-  const int ea = lane / 6, eb2 = lane % 6, fa = (32 + lane) / 6, fb = (32 + lane) % 6;
-  // GE (288 MB at 1M observations) comes from DRAM: the lines of a landmark (K x 288 B) are prefetched into L1 one
-  // landmark ahead, otherwise every first touch inside the pair walk is an exposed ~1 us miss
-  int t0n = 0, Kn = 0;
-  if (gwarp < A.n_points) { t0n = A.pt_start[gwarp]; Kn = A.pt_start[gwarp + 1] - t0n; }
-  { const char *pf = reinterpret_cast<const char *>(GE + 36 * (size_t)t0n) + 128 * lane;
-    if (128 * lane < 288 * Kn) asm volatile("prefetch.global.L1 [%0];" :: "l"(pf)); if (128 * (lane + 32) < 288 * Kn) asm volatile("prefetch.global.L1 [%0];" :: "l"(pf + 4096)); }
-  for (int j = gwarp; j < A.n_points; j += nwarps) {
-    const int t0 = t0n, K = Kn;
-    if (j + nwarps < A.n_points) {
-      t0n = A.pt_start[j + nwarps]; Kn = A.pt_start[j + nwarps + 1] - t0n;
-      const char *pf = reinterpret_cast<const char *>(GE + 36 * (size_t)t0n) + 128 * lane;
-      if (128 * lane < 288 * Kn) asm volatile("prefetch.global.L1 [%0];" :: "l"(pf)); if (128 * (lane + 32) < 288 * Kn && Kn <= 32) asm volatile("prefetch.global.L1 [%0];" :: "l"(pf + 4096));
+// ---- co-visibility lists of the camera blocks, built once per problem (omvg_ba_create).  For every landmark the
+// stage / gather pair takes (one intrinsic group, 1..32 observations) they hold the observation pairs (t, u) with
+// cam(u) >= cam(t), keyed by the BSR index of block (cam(t), cam(u)); a stable sort by key lists the pairs of every
+// upper and diagonal block in landmark order.  Outlier rejection and omvg_ba_remove_points only set weights to 0 and
+// make landmarks constant: their H records become zero and the lists stay valid without a rebuild.
+__device__ __forceinline__ bool gather_point(const int *__restrict__ pt_start, const unsigned char *__restrict__ pt_single, int j) {
+  const int K = pt_start[j + 1] - pt_start[j];
+  return pt_single[j] != 0 && K > 0 && K <= 32;
+}
+__global__ void pair_count_kernel(const int *__restrict__ pt_start, const unsigned char *__restrict__ pt_single, const int *__restrict__ obs_pose,
+                                  int n_points, long long *__restrict__ count) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x; if (j >= n_points) return;
+  long long k = 0;
+  if (gather_point(pt_start, pt_single, j))
+    for (int t = pt_start[j]; t < pt_start[j + 1]; ++t) for (int u = pt_start[j]; u < pt_start[j + 1]; ++u) k += obs_pose[u] >= obs_pose[t];
+  count[j] = k;
+}
+__global__ void pair_emit_kernel(const int *__restrict__ pt_start, const unsigned char *__restrict__ pt_single, const int *__restrict__ obs_pose,
+                                 int n_points, const long long *__restrict__ offset, Bsr B, int *__restrict__ key, int2 *__restrict__ pair) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x; if (j >= n_points || !gather_point(pt_start, pt_single, j)) return;
+  long long k = offset[j];
+  for (int t = pt_start[j]; t < pt_start[j + 1]; ++t) {
+    const int ct = obs_pose[t];
+    for (int u = pt_start[j]; u < pt_start[j + 1]; ++u) {
+      const int cu = obs_pose[u]; if (cu < ct) continue;
+      key[k] = bsr_find(B, ct, cu); pair[k] = make_int2(t, u); ++k;
     }
-    if (K == 0 || K > 32 || !A.pt_single[j]) continue;
-    const int cam_l = lane < K ? A.obs_pose[t0 + lane] : 0;
-    const unsigned lowmask = (1u << (cam_l & 31)) - 1u;
-    int rp = 0, wp = 0; unsigned bm = 0;
-    { const int c0 = __shfl_sync(0xffffffffu, cam_l, 0); const size_t w = (size_t)c0 * A.bsr.words + (cam_l >> 5); rp = A.bsr.rowptr[c0]; wp = A.bsr.wprefix[w]; bm = A.bsr.bitmap[w]; }
-    const double *ge = GE + 36 * (size_t)t0;
-    for (int tt = 0; tt < K; ++tt) {
-      const int ctt = __shfl_sync(0xffffffffu, cam_l, tt);
-      const int cur = (lane < K && cam_l >= ctt) ? rp + wp + __popc(bm & lowmask) : -1;
-      if (tt + 1 < K) { const int cn = __shfl_sync(0xffffffffu, cam_l, tt + 1); const size_t w = (size_t)cn * A.bsr.words + (cam_l >> 5); rp = A.bsr.rowptr[cn]; wp = A.bsr.wprefix[w]; bm = A.bsr.bitmap[w]; }
-      const double *gt = ge + 36 * tt;
-      const double g0 = gt[ea], g1 = gt[6 + ea], g2 = gt[12 + ea];
-      const double h0 = lane < 4 ? gt[fa] : 0.0, h1 = lane < 4 ? gt[6 + fa] : 0.0, h2 = lane < 4 ? gt[12 + fa] : 0.0;
-      unsigned todo = __ballot_sync(0xffffffffu, cur >= 0);
-      while (todo) {
-        const int u = __ffs(todo) - 1; todo &= todo - 1;
-        const int bi = __shfl_sync(0xffffffffu, cur, u);
-        double *blk = A.Scc + 36 * (size_t)bi;
-        const double *ef = ge + 36 * u + 18;
-        atomicAdd(blk + lane, -(g0 * ef[eb2] + g1 * ef[6 + eb2] + g2 * ef[12 + eb2]));
-        if (lane < 4) atomicAdd(blk + 32 + lane, -(h0 * ef[fb] + h1 * ef[6 + fb] + h2 * ef[12 + fb]));
+  }
+}
+
+// Scc of the gather path: one warp per chunk of at most GATHER_CHUNK pairs of one block.  Chunks are numbered in block
+// (= camera row) order, so the warps of a CTA mostly read the H records of one camera row.  Six lanes take one pair,
+// lane i of them row i of  H_t' H_u  (column i of H_t, all of H_u as nine 16-byte loads), and five pairs go at once
+// (lanes 30, 31 idle): 2.4 load instructions per pair.  (Lane e summing element e of the block took 12 per pair and
+// was bound by load issue: 0.67 ms per LM step on config 2, H100 SXM at 700 W.)  Each group of six sums its pairs in list order; the five
+// groups are added in group order, so the result does not depend on scheduling.  A block of one chunk is stored
+// directly.  The chunks of a longer list store partial sums in `part`; the last of them to finish (counted in
+// `ticket`, which it resets) adds the partials in chunk order.  An upper block is stored with its transpose, a diagonal
+// block as Fc'Fc - sum.
+constexpr int GATHER_CHUNK = 120;                   // pairs per warp (a multiple of the 30 a warp loads at once)
+struct GatherArgs {
+  const double *H, *FtF; const int2 *pair; const int *pair_start, *chunk_blk, *chunk_first, *brow, *cols; Bsr bsr;
+  double *Scc, *part; int *ticket; int n_chunks;
+};
+__global__ void __launch_bounds__(256) schur_gather_kernel(GatherArgs G) {
+  const unsigned FULL = 0xffffffffu;
+  const int lane = threadIdx.x & 31, ch = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (ch >= G.n_chunks) return;
+  const int e = G.chunk_blk[ch], c0 = G.chunk_first[e], nch = G.chunk_first[e + 1] - c0;
+  const int begin = G.pair_start[e] + (ch - c0) * GATHER_CHUNK, end = min(begin + GATHER_CHUNK, G.pair_start[e + 1]);
+  const int grp = lane / 6, i = lane - 6 * grp;     // lanes 30, 31: group 5, no pair
+  double s[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  for (int p0 = begin; p0 < end; p0 += 30) {
+    const int np = min(30, end - p0);
+    const int2 pr = lane < np ? G.pair[p0 + lane] : make_int2(0, 0);
+    #pragma unroll 2
+    for (int g = 0; g < np; g += 5) {
+      const int q = g + grp;
+      const int t = __shfl_sync(FULL, pr.x, q & 31), u = __shfl_sync(FULL, pr.y, q & 31);
+      if (grp < 5 && q < np) {
+        const double *ht = G.H + HREC * (size_t)t;
+        const double2 *hu = reinterpret_cast<const double2 *>(G.H + HREC * (size_t)u);
+        const double a0 = __ldg(ht + i), a1 = __ldg(ht + 6 + i), a2 = __ldg(ht + 12 + i);
+        double b[18];
+        #pragma unroll
+        for (int m = 0; m < 9; ++m) { const double2 v = __ldg(hu + m); b[2 * m] = v.x; b[2 * m + 1] = v.y; }
+        #pragma unroll
+        for (int k = 0; k < 6; ++k) s[k] += a0 * b[k] + a1 * b[6 + k] + a2 * b[12 + k];
       }
     }
+  }
+  #pragma unroll
+  for (int g = 1; g < 5; ++g)                       // groups 1..4 into group 0, in group order
+    #pragma unroll
+    for (int k = 0; k < 6; ++k) { const double v = __shfl_sync(FULL, s[k], (lane + 6 * g) & 31); if (grp == 0) s[k] += v; }
+  if (nch > 1) {
+    if (grp == 0) {
+      #pragma unroll
+      for (int k = 0; k < 6; ++k) G.part[36 * (size_t)ch + 6 * i + k] = s[k];
+    }
+    __threadfence();
+    __syncwarp();
+    int last = 0;
+    if (lane == 0) last = atomicAdd(&G.ticket[e], 1) == nch - 1;
+    if (!__shfl_sync(FULL, last, 0)) return;
+    __threadfence();
+    if (grp == 0) {
+      #pragma unroll
+      for (int k = 0; k < 6; ++k) s[k] = 0.0;
+      for (int c = c0; c < c0 + nch; ++c) {
+        #pragma unroll
+        for (int k = 0; k < 6; ++k) s[k] += __ldcg(G.part + 36 * (size_t)c + 6 * i + k);
+      }
+    }
+    if (lane == 0) G.ticket[e] = 0;
+  }
+  if (grp != 0) return;
+  const int a = G.brow[e], b = G.cols[e];
+  double *dst = G.Scc + 36 * (size_t)e;
+  if (a == b) {
+    const double *f = G.FtF + 36 * (size_t)a + 6 * i;
+    #pragma unroll
+    for (int k = 0; k < 6; ++k) dst[6 * i + k] = f[k] - s[k];
+  } else {
+    double *tr = G.Scc + 36 * (size_t)bsr_find(G.bsr, b, a);
+    #pragma unroll
+    for (int k = 0; k < 6; ++k) { dst[6 * i + k] = -s[k]; tr[6 * k + i] = -s[k]; }
   }
 }
 
