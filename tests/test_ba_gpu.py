@@ -84,7 +84,8 @@ def test_multiple_intrinsic_groups(ba, n_intr, model):
 
 
 def test_pcg_variants_agree(ba, monkeypatch):
-    """Two-level block-PCG (default) and plain block-Jacobi PCG with the border inside the iteration."""
+    """Two-level block-PCG (default: intrinsics border eliminated blockwise) and pcg_kernel (forced by OMVG_BA_PCG1:
+    the border inside the iteration, the same aggregated coarse space on the camera rows)."""
     monkeypatch.setenv("OMVG_BA_DENSE_MAX", "0"); monkeypatch.setenv("OMVG_BA_DENSE2_MAX", "0")     # (40 cameras would be solved directly)
     s = synth.ba_scene(40, 2000, 8, seed=12)
     a = ba.solve(s)
@@ -98,8 +99,9 @@ def test_context_reset_is_reproducible(ba):
     s = synth.ba_scene(20, 1000, 6, seed=2)
     ctx = ba.BAContext(s)
     a = ctx.run(); ctx.reset(); b = ctx.run()
-    # cost/gradient/model reductions are fixed-order; the Schur accumulation uses FP64 atomics, so two
-    # runs agree to rounding (not bitwise)
+    # cost/gradient/model reductions and the camera blocks of the Schur complement are fixed-order; the border, its
+    # right-hand side and the landmarks outside the co-visibility lists use FP64 atomics, so two runs agree to
+    # rounding (not bitwise)
     assert abs(a["final_cost"] - b["final_cost"]) <= 1e-12 * a["final_cost"] and a["iterations"] == b["iterations"]
     ctx.close()
 
@@ -318,21 +320,38 @@ def test_remove_points_on_resident_scene(ba):
     assert abs(b["final_cost"] - o["final_cost"]) <= 1e-7 * o["final_cost"] and b["iterations"] == o["iterations"]
 
 
+def _one_pose_scene(n_views=6, n_points=300, seed=9):
+    """n_views views on ONE pose, each with its own intrinsic group (focal 1000 .. 1100): observations re-projected
+    through the oracle at the initial parameters, plus 0.5 px noise; then the landmarks are perturbed."""
+    s = synth.ba_scene(n_views, n_points, 4, seed=seed)
+    intr = np.repeat(s["intrinsics"][:1], n_views, axis=0); intr[:, 0] += 20.0 * np.arange(n_views)
+    s.update(poses=np.ascontiguousarray(s["poses"][:1]), intrinsics=np.ascontiguousarray(intr), intr_model=np.full(n_views, 1, np.int32),
+             view_pose=np.zeros(n_views, np.int32), view_intr=np.arange(n_views, dtype=np.int32), obs_xy=np.zeros_like(s["obs_xy"]))
+    proj = ck.oracle_ba_eval(s, use_loss=0)[1]                  # residual = projection - observation (0)
+    rng = np.random.default_rng(seed)
+    s["obs_xy"] = np.ascontiguousarray(proj + rng.normal(0, 0.5, proj.shape))
+    s["points"] = np.ascontiguousarray(s["points"] + rng.normal(0, 0.01, s["points"].shape))
+    return s
+
+
 def test_direct_and_iterative_reduced_solves_agree(ba, monkeypatch):
     """Up to 220 reduced unknowns one CTA solves the reduced camera system directly (dense L D L', as Ceres' Cholesky does),
     up to 640 it is inverted explicitly (blocked Gauss-Jordan over all SMs); above, and with OMVG_BA_DENSE_MAX=0 /
-    OMVG_BA_DENSE2_MAX=0, the two-level PCG runs.  Same LM trajectory either way."""
-    for cams, model in ((12, 1), (30, 3), (35, 1), (50, 1), (80, 2)):   # 6 * 35 + 8 = 218 unknowns <= 220: one CTA; up to 640: explicit inverse
-        s = synth.ba_scene(cams, 60 * cams, 8, seed=5 + cams, model=model)
+    OMVG_BA_DENSE2_MAX=0, the two-level PCG runs (on one CTA up to 12 poses; without a coarse space on one pose).
+    Same LM trajectory either way."""
+    cases = [(cams, synth.ba_scene(cams, 60 * cams, 8, seed=5 + cams, model=model), {})
+             for cams, model in ((12, 1), (30, 3), (35, 1), (50, 1), (80, 2))]   # 6 * 35 + 8 = 218 unknowns <= 220: one CTA; up to 640: explicit inverse
+    cases.append(("one pose", _one_pose_scene(), dict(pcg_tolerance=1e-12)))   # (block-Jacobi alone on an ill-posed scene)
+    for name, s, kw in cases:
         monkeypatch.delenv("OMVG_BA_DENSE_MAX", raising=False); monkeypatch.delenv("OMVG_BA_DENSE2_MAX", raising=False)
-        a = ba.solve(s)
+        a = ba.solve(s, **kw)
         monkeypatch.setenv("OMVG_BA_DENSE_MAX", "0"); monkeypatch.setenv("OMVG_BA_DENSE2_MAX", "0")
-        b = ba.solve(s)
-        assert a["pcg_iterations"] == 0 and b["pcg_iterations"] > 0, (cams, a["pcg_iterations"], b["pcg_iterations"])
-        assert a["iterations"] == b["iterations"]
-        assert abs(a["final_cost"] - b["final_cost"]) <= 1e-8 * a["final_cost"]
+        b = ba.solve(s, **kw)
+        assert a["pcg_iterations"] == 0 and b["pcg_iterations"] > 0, (name, a["pcg_iterations"], b["pcg_iterations"])
+        assert a["iterations"] == b["iterations"], name
+        assert abs(a["final_cost"] - b["final_cost"]) <= 1e-8 * a["final_cost"], name
         o = ck.oracle_ba_solve(s)
-        assert abs(a["final_cost"] - o["final_cost"]) <= 1e-9 * o["final_cost"] and a["iterations"] == o["iterations"], (a["final_cost"], o["final_cost"])
+        assert abs(a["final_cost"] - o["final_cost"]) <= 1e-9 * o["final_cost"] and a["iterations"] == o["iterations"], (name, a["final_cost"], o["final_cost"])
 
 
 def test_tight_pcg_reproduces_oracle_to_rounding(ba, monkeypatch):
@@ -349,8 +368,8 @@ def test_tight_pcg_reproduces_oracle_to_rounding(ba, monkeypatch):
 
 @pytest.mark.parametrize("cfg", [(40, 120, 36), (64, 50, 64)])
 def test_many_observations_per_landmark(ba, cfg):
-    """Landmarks with more than 32 observations take the per-observation Schur kernel (the warp-per-landmark
-    kernel stages at most 32): both paths in one solve."""
+    """Landmarks with more than 32 observations take the per-observation Schur kernel (the co-visibility lists hold
+    landmarks of at most 32 views): both paths in one solve."""
     s = synth.ba_scene(*cfg, seed=2)
     extra = synth.ba_scene(cfg[0], 400, 5, seed=3)             # plus ordinary short tracks
     n0 = len(s["points"])

@@ -32,7 +32,7 @@ def gpu_info() -> dict:
 
 
 def short(name: str) -> str:
-    """'void omvg::ba::schur_stage_kernel<3, 5>(omvg::ba::SchurArgs, ...)' -> 'schur_stage_kernel<3, 5>'"""
+    """'void omvg::ba::schur_stage_kernel<3>(omvg::ba::SchurArgs, ...)' -> 'schur_stage_kernel<3>'"""
     name = re.sub(r"^void ", "", name.split("(")[0])
     return re.sub(r"^(omvg::)?(ba::)?(\(anonymous namespace\)::)?", "", name)
 
