@@ -160,6 +160,24 @@ int omvg_geom_fundamental_acransac(int device, uint64_t n_pairs, const uint64_t 
 int omvg_geom_acransac(int device, int32_t model, uint64_t n_pairs, const uint64_t *offsets, const double *xI, const double *xJ,
                        const int32_t *image_size, double precision, uint32_t max_iterations,
                        uint32_t *inliers, uint32_t *n_inliers, double *F, double *stats);
+/* The essential-matrix model of calibrated pinhole views: GeometricFilter_EMatrix_AC::Robust_estimation
+ * (matching_image_collection/E_ACRobust.hpp:55-150), i.e. ACKernelAdaptorEssential<FivePointSolver,
+ * EpipolarDistanceError> + ACRANSAC.  Samples of 5 matches are solved on the bearing vectors normalize(K^-1 [x; 1]) by
+ * the five-point solver (up to 10 models per sample); each model is scored on the PIXEL positions with the
+ * point-to-line error against F = K_J^-T E K_I^-1, without normalisation.  omvg_geom_acransac rejects this model: it
+ * has no intrinsics argument.
+ *   intr[n_pairs][6]          {f_I, ppx_I, ppy_I, f_J, ppx_J, ppy_J}: K = [[f, 0, ppx], [0, f, ppy], [0, 0, 1]]
+ *                             (Pinhole_Intrinsic::K()); f finite and > 0, principal points finite
+ * Other arguments as omvg_geom_fundamental_acransac.  out: E[n_pairs][9] row-major as ACRANSAC leaves it (x_J' E x_I = 0
+ * on bearings), stats[n_pairs][2] = {errorMax in SQUARED pixels (the reference's unormalizeError is the identity here),
+ * minNFA}; the reference keeps the pair iff n_inliers > 2.5 * 5. */
+#define OMVG_GEOM_ESSENTIAL   2
+int omvg_geom_essential_acransac(int device, uint64_t n_pairs, const uint64_t *offsets, const double *xI, const double *xJ,
+                                 const int32_t *image_size, const double *intr, double precision, uint32_t max_iterations,
+                                 uint32_t *inliers, uint32_t *n_inliers, double *E, double *stats);
+/* Validation aid (tests only): the device five-point solver on n independent samples of 5 bearing pairs.
+ * b1, b2 [n][5][3]; out: E[n][10][9] (the first n_models[s] rows of sample s are its real solutions, row-major). */
+int omvg_geom_debug_five_point(int device, uint32_t n, const double *b1, const double *b2, double *E, int32_t *n_models);
 
 /* ===================================================================== BA ================= */
 #define OMVG_BA_INTR_STRIDE 8   /* doubles reserved per intrinsic block */

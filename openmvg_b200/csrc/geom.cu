@@ -1,4 +1,4 @@
-// geom.cu — per-pair a-contrario RANSAC (fundamental-matrix model) on sm_100a: the geometric filter openMVG runs
+// geom.cu — per-pair a-contrario RANSAC (fundamental-matrix, homography and essential-matrix models) on sm_90a: the geometric filter openMVG runs
 // right after putative matching (SURVEY §8f N4).
 //
 // Replaces (reference, $OPENMVG/src/openMVG):
@@ -19,6 +19,7 @@
 
 #include <cfloat>
 #include <cmath>
+#include <type_traits>
 #include <vector>
 
 namespace omvg { namespace geom {
@@ -129,6 +130,7 @@ struct Args {
   uint32_t *inliers;                       // out [n_matches]: first n_inliers[p] entries of pair p's segment
   uint32_t *n_inliers; double *F; double *stats;
   unsigned int n_pairs;
+  const double *intr;                      // essential model: [n_pairs][6] f, ppx, ppy of view I then view J
 };
 
 struct Smem {
@@ -140,6 +142,357 @@ struct Smem {
   int n_models, better_now;
   double nfa_thr, nfa_val;                 // threshold / NFA of the model being accepted
 };
+
+// ---------------------------------------------------------------- essential model: the five-point solver (DESIGN §3.8)
+// multiview/solver_essential_five_point.cpp:35-214, restated step by step as the CPU restatement used by the tests (essential_oracle.cpp) does it (same
+// algorithms, same operation order per entry).  One warp solves one sample; every row- or column-parallel loop is spread
+// over the lanes, the scalar control flow runs redundantly in all lanes, and shared scalars are written by lane 0.
+struct FivePointWork {
+  double AtA[9][9], V[9][9], basis[9][4];  // A'A of the 5 epipolar rows, Jacobi vectors, the 4-D null space (E_ij = row 3i+j)
+  double L[6][10], C[10][20], f[10];       // E E' - tr/2 (packed upper), the 10x20 constraint matrix, elimination factors
+  double At[10][10], H[10][10];            // the action matrix and its Hessenberg / quasi-triangular form
+  double models[10][9];                    // real solutions, row-major (b2' E b1 = 0)
+  int n_models;
+};
+
+// Polynomials in (x, y, z), monomials in the order of Stewenius et al. (cubic 0-9, quadratic 10-15, x y z 16-18, 1 19);
+// a linear polynomial is held as (x y z 1), a quadratic as its 10 trailing coefficients.
+__device__ void poly_lin_lin(const double a[4], const double b[4], double r[10]) {
+  r[0] = a[0] * b[0];
+  r[1] = a[0] * b[1] + a[1] * b[0];
+  r[2] = a[1] * b[1];
+  r[3] = a[0] * b[2] + a[2] * b[0];
+  r[4] = a[1] * b[2] + a[2] * b[1];
+  r[5] = a[2] * b[2];
+  r[6] = a[0] * b[3] + a[3] * b[0];
+  r[7] = a[1] * b[3] + a[3] * b[1];
+  r[8] = a[2] * b[3] + a[3] * b[2];
+  r[9] = a[3] * b[3];
+}
+__device__ void poly_quad_lin(const double a[10], const double b[4], double r[20]) {
+  const double xx = a[0], xy = a[1], yy = a[2], xz = a[3], yz = a[4], zz = a[5], x = a[6], y = a[7], z = a[8], o = a[9];
+  const double bx = b[0], by = b[1], bz = b[2], bo = b[3];
+  r[0] = xx * bx;
+  r[1] = xx * by + xy * bx;
+  r[2] = xy * by + yy * bx;
+  r[3] = yy * by;
+  r[4] = xx * bz + xz * bx;
+  r[5] = xy * bz + yz * bx + xz * by;
+  r[6] = yy * bz + yz * by;
+  r[7] = xz * bz + zz * bx;
+  r[8] = yz * bz + zz * by;
+  r[9] = zz * bz;
+  r[10] = xx * bo + x * bx;
+  r[11] = xy * bo + x * by + y * bx;
+  r[12] = yy * bo + y * by;
+  r[13] = xz * bo + x * bz + z * bx;
+  r[14] = yz * bo + y * bz + z * by;
+  r[15] = zz * bo + z * bz;
+  r[16] = x * bo + o * bx;
+  r[17] = y * bo + o * by;
+  r[18] = z * bo + o * bz;
+  r[19] = o * bo;
+}
+
+// Francis double-shift QR (EISPACK hqr: exceptional shifts at 10 and 20 iterations, 30 n iterations in all) on the
+// Hessenberg matrix a (eigenvalues only).  Called by the whole warp; wr/wi end up the same in every lane.
+__device__ bool hessenberg_qr_warp(double (*a)[10], double wr[10], double wi[10], int lane) {
+  const int n = 10;
+  double anorm = 0;
+  for (int i = 0; i < n; ++i) for (int j = i > 0 ? i - 1 : 0; j < n; ++j) anorm += fabs(a[i][j]);
+  int nn = n - 1, itn = 30 * n;
+  double t = 0;
+  while (nn >= 0) {
+    int its = 0, l;
+    do {
+      for (l = nn; l >= 1; --l) {
+        double s = fabs(a[l - 1][l - 1]) + fabs(a[l][l]);
+        if (s == 0.0) s = anorm;
+        if (fabs(a[l][l - 1]) + s == s) break;
+      }
+      __syncwarp();
+      if (l >= 1 && lane == 0) a[l][l - 1] = 0.0;
+      __syncwarp();
+      double x = a[nn][nn];
+      if (l == nn) { wr[nn] = x + t; wi[nn] = 0.0; --nn; continue; }
+      double y = a[nn - 1][nn - 1], w = a[nn][nn - 1] * a[nn - 1][nn];
+      if (l == nn - 1) {
+        const double p = 0.5 * (y - x), q = p * p + w;
+        double z = sqrt(fabs(q));
+        x += t;
+        if (q >= 0.0) {
+          z = p + (p >= 0 ? z : -z);
+          wr[nn - 1] = wr[nn] = x + z;
+          if (z != 0.0) wr[nn] = x - w / z;
+          wi[nn - 1] = wi[nn] = 0.0;
+        } else {
+          wr[nn - 1] = wr[nn] = x + p;
+          wi[nn - 1] = -z; wi[nn] = z;
+        }
+        nn -= 2;
+        continue;
+      }
+      if (itn == 0) return false;
+      if (its == 10 || its == 20) {
+        t += x;
+        __syncwarp();
+        if (lane <= nn) a[lane][lane] -= x;
+        __syncwarp();
+        const double s = fabs(a[nn][nn - 1]) + fabs(a[nn - 1][nn - 2]);
+        y = x = 0.75 * s;
+        w = -0.4375 * s * s;
+      }
+      ++its; --itn;
+      int m;
+      double p = 0, q = 0, r = 0, z;
+      for (m = nn - 2; m >= l; --m) {
+        z = a[m][m];
+        r = x - z;
+        double s = y - z;
+        p = (r * s - w) / a[m + 1][m] + a[m][m + 1];
+        q = a[m + 1][m + 1] - z - r - s;
+        r = a[m + 2][m + 1];
+        s = fabs(p) + fabs(q) + fabs(r);
+        p /= s; q /= s; r /= s;
+        if (m == l) break;
+        const double u = fabs(a[m][m - 1]) * (fabs(q) + fabs(r));
+        const double v = fabs(p) * (fabs(a[m - 1][m - 1]) + fabs(z) + fabs(a[m + 1][m + 1]));
+        if (u + v == v) break;
+      }
+      __syncwarp();
+      if (lane >= m + 2 && lane <= nn) { a[lane][lane - 2] = 0.0; if (lane != m + 2) a[lane][lane - 3] = 0.0; }
+      __syncwarp();
+      for (int k = m; k <= nn - 1; ++k) {
+        if (k != m) {
+          p = a[k][k - 1]; q = a[k + 1][k - 1]; r = 0.0;
+          if (k != nn - 1) r = a[k + 2][k - 1];
+          x = fabs(p) + fabs(q) + fabs(r);
+          if (x != 0.0) { p /= x; q /= x; r /= x; }
+        }
+        const double sq = sqrt(p * p + q * q + r * r), s = p >= 0 ? sq : -sq;
+        if (s == 0.0) continue;
+        __syncwarp();
+        if (lane == 0) {
+          if (k == m) { if (l != m) a[k][k - 1] = -a[k][k - 1]; }
+          else a[k][k - 1] = -s * x;
+        }
+        p += s; x = p / s; y = q / s; z = r / s; q /= p; r /= p;
+        __syncwarp();
+        if (lane >= k && lane <= nn) {             // rows k..k+2, one column per lane
+          const int j = lane;
+          double pp = a[k][j] + q * a[k + 1][j];
+          if (k != nn - 1) { pp += r * a[k + 2][j]; a[k + 2][j] -= pp * z; }
+          a[k + 1][j] -= pp * y; a[k][j] -= pp * x;
+        }
+        __syncwarp();
+        const int mmin = nn < k + 3 ? nn : k + 3;
+        if (lane >= l && lane <= mmin) {           // columns k..k+2, one row per lane
+          const int i = lane;
+          double pp = x * a[i][k] + y * a[i][k + 1];
+          if (k != nn - 1) { pp += z * a[i][k + 2]; a[i][k + 2] -= pp * r; }
+          a[i][k + 1] -= pp * q; a[i][k] -= pp;
+        }
+        __syncwarp();
+      }
+    } while (l < nn - 1);
+  }
+  return true;
+}
+
+// b1, b2: bearing vectors [.][3]; sample: the 5 indices.  Called by all 32 lanes of one warp; W.models / W.n_models out.
+__device__ void five_point_warp(FivePointWork &W, const double *b1, const double *b2, const uint32_t *sample, int lane) {
+  for (int e = lane; e < 81; e += 32) {                                   // A'A, EncodeEpipolarEquation rows
+    const int i = e / 9, j = e % 9;
+    double acc = 0;
+    for (int t = 0; t < 5; ++t) {
+      const size_t s = sample[t];
+      acc += (b2[3 * s + i / 3] * b1[3 * s + i % 3]) * (b2[3 * s + j / 3] * b1[3 * s + j % 3]);
+    }
+    W.AtA[i][j] = acc;
+    W.V[i][j] = i == j ? 1.0 : 0.0;
+  }
+  __syncwarp();
+  double (*A)[9] = W.AtA, (*V)[9] = W.V;
+  for (int sweep = 0; sweep < 60; ++sweep) {                              // cyclic Jacobi, the 9 k-updates over lanes
+    double off = 0, diag = 0;
+    for (int i = 0; i < 9; ++i) { diag += A[i][i] * A[i][i]; for (int j = i + 1; j < 9; ++j) off += A[i][j] * A[i][j]; }
+    if (off <= 1e-60 * diag || off == 0.0) break;
+    for (int p = 0; p < 8; ++p)
+      for (int q = p + 1; q < 9; ++q) {
+        const double apq = A[p][q];
+        if (apq == 0.0) continue;
+        const double theta = (A[q][q] - A[p][p]) / (2.0 * apq);
+        const double t = (theta >= 0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+        __syncwarp();
+        if (lane < 9) { const int k = lane; const double akp = A[k][p], akq = A[k][q]; A[k][p] = c * akp - s * akq; A[k][q] = s * akp + c * akq; }
+        __syncwarp();
+        if (lane < 9) {
+          const int k = lane;
+          const double apk = A[p][k], aqk = A[q][k]; A[p][k] = c * apk - s * aqk; A[q][k] = s * apk + c * aqk;
+          const double vkp = V[k][p], vkq = V[k][q]; V[k][p] = c * vkp - s * vkq; V[k][q] = s * vkp + c * vkq;
+        }
+        __syncwarp();
+      }
+  }
+  {                                                                        // the 4 smallest, ascending
+    unsigned used = 0;
+    for (int c = 0; c < 4; ++c) {
+      int best = -1;
+      for (int i = 0; i < 9; ++i) if (!(used >> i & 1u) && (best < 0 || A[i][i] < A[best][best])) best = i;
+      used |= 1u << best;
+      if (lane < 9) W.basis[lane][c] = V[lane][best];
+    }
+  }
+  __syncwarp();
+  const double (*E)[4] = W.basis;
+  if (lane < 6) {                                                          // E E' (upper), one entry per lane
+    const int P0[6] = {0, 0, 0, 1, 1, 2}, P1[6] = {0, 1, 2, 1, 2, 2};
+    const int i = P0[lane], j = P1[lane];
+    double t[10];
+    poly_lin_lin(E[3 * i], E[3 * j], W.L[lane]);
+    for (int k = 1; k < 3; ++k) { poly_lin_lin(E[3 * i + k], E[3 * j + k], t); for (int c = 0; c < 10; ++c) W.L[lane][c] += t[c]; }
+  }
+  __syncwarp();
+  if (lane < 10) {
+    const int c = lane;
+    const double half_trace = 0.5 * (W.L[0][c] + W.L[3][c] + W.L[5][c]);
+    W.L[0][c] -= half_trace; W.L[3][c] -= half_trace; W.L[5][c] -= half_trace;
+  }
+  __syncwarp();
+  if (lane == 0) {                                                         // det E = 0
+    const int T[3][4] = {{1, 5, 2, 4}, {2, 3, 0, 5}, {0, 4, 1, 3}};
+    double *row = W.C[0];
+    for (int c = 0; c < 20; ++c) row[c] = 0;
+    for (int c = 0; c < 3; ++c) {
+      double u[10], v[10], w[20];
+      poly_lin_lin(E[T[c][0]], E[T[c][1]], u); poly_lin_lin(E[T[c][2]], E[T[c][3]], v);
+      for (int k = 0; k < 10; ++k) u[k] -= v[k];
+      poly_quad_lin(u, E[6 + c], w);
+      for (int k = 0; k < 20; ++k) row[k] += w[k];
+    }
+  } else if (lane < 10) {                                                  // (E E' - tr/2) E = 0, one row per lane
+    const int S3[3][3] = {{0, 1, 2}, {1, 3, 4}, {2, 4, 5}};
+    const int i = (lane - 1) / 3, j = (lane - 1) % 3;
+    double *row = W.C[lane], w[20];
+    poly_quad_lin(W.L[S3[i][0]], E[j], row);
+    for (int k = 1; k < 3; ++k) { poly_quad_lin(W.L[S3[i][k]], E[3 * k + j], w); for (int c = 0; c < 20; ++c) row[c] += w[c]; }
+  }
+  __syncwarp();
+  double (*C)[20] = W.C;
+  for (int k = 0; k < 10; ++k) {                                           // Gauss-Jordan, partial pivoting, one column per lane
+    int piv = k;
+    for (int r = k + 1; r < 10; ++r) if (fabs(C[r][k]) > fabs(C[piv][k])) piv = r;
+    __syncwarp();
+    if (piv != k && lane < 20) { const double a = C[k][lane]; C[k][lane] = C[piv][lane]; C[piv][lane] = a; }
+    __syncwarp();
+    if (lane < 10) W.f[lane] = lane == k ? 0.0 : C[lane][k] / C[k][k];
+    __syncwarp();
+    if (lane >= k && lane < 20) for (int r = 0; r < 10; ++r) if (r != k) C[r][lane] -= W.f[r] * C[k][lane];
+    __syncwarp();
+  }
+  for (int e = lane; e < 100; e += 32) {                                   // the action matrix
+    const int r = e / 10, c = e % 10;
+    const int R[6] = {0, 1, 2, 4, 5, 7};
+    double v = 0.0;
+    if (r < 6) v = C[R[r]][10 + c] / C[R[r]][R[r]];
+    else if ((r == 6 && c == 0) || (r == 7 && c == 1) || (r == 8 && c == 3) || (r == 9 && c == 6)) v = -1.0;
+    W.At[r][c] = v; W.H[r][c] = v;
+  }
+  __syncwarp();
+  double (*a)[10] = W.H;
+  for (int m = 1; m < 9; ++m) {                                            // Householder reduction to Hessenberg form
+    double scale = 0;
+    for (int i = m; i < 10; ++i) scale += fabs(a[i][m - 1]);
+    if (scale == 0.0) continue;
+    double u[10], h = 0;
+    for (int i = 9; i >= m; --i) { u[i] = a[i][m - 1] / scale; h += u[i] * u[i]; }
+    const double g = u[m] > 0 ? -sqrt(h) : sqrt(h);
+    h -= u[m] * g; u[m] -= g;
+    if (lane >= m && lane < 10) {                                          // (I - u u'/h) A, one column per lane
+      const int j = lane;
+      double f = 0;
+      for (int i = 9; i >= m; --i) f += u[i] * a[i][j];
+      f /= h;
+      for (int i = m; i < 10; ++i) a[i][j] -= f * u[i];
+    }
+    __syncwarp();
+    if (lane < 10) {                                                       // A (I - u u'/h), one row per lane
+      const int i = lane;
+      double f = 0;
+      for (int j = 9; j >= m; --j) f += u[j] * a[i][j];
+      f /= h;
+      for (int j = m; j < 10; ++j) a[i][j] -= f * u[j];
+    }
+    __syncwarp();
+    if (lane == 0) { a[m][m - 1] = scale * g; for (int i = m + 1; i < 10; ++i) a[i][m - 1] = 0.0; }
+    __syncwarp();
+  }
+  double wr[10], wi[10];
+  const bool ok = hessenberg_qr_warp(a, wr, wi, lane);
+  // one real eigenvalue per lane: null vector of At - lambda I (complete pivoting, last unknown = 1), E = basis * v[6..9]
+  const bool real = ok && lane < 10 && wi[lane < 10 ? lane : 0] == 0.0;
+  const unsigned bal = __ballot_sync(0xffffffffu, real);
+  if (real) {
+    const double lambda = wr[lane];
+    double M[10][10], y[10], v[10]; int cp[10];
+    for (int i = 0; i < 10; ++i) { cp[i] = i; for (int j = 0; j < 10; ++j) M[i][j] = W.At[i][j] - (i == j ? lambda : 0.0); }
+    for (int k = 0; k < 9; ++k) {
+      int pr = k, pc = k;
+      for (int r = k; r < 10; ++r) for (int c = k; c < 10; ++c) if (fabs(M[r][c]) > fabs(M[pr][pc])) { pr = r; pc = c; }
+      if (pr != k) for (int c = 0; c < 10; ++c) { const double tmp = M[k][c]; M[k][c] = M[pr][c]; M[pr][c] = tmp; }
+      if (pc != k) { for (int r = 0; r < 10; ++r) { const double tmp = M[r][k]; M[r][k] = M[r][pc]; M[r][pc] = tmp; } const int ti = cp[k]; cp[k] = cp[pc]; cp[pc] = ti; }
+      for (int r = k + 1; r < 10; ++r) {
+        const double f = M[r][k] / M[k][k];
+        for (int c = k; c < 10; ++c) M[r][c] -= f * M[k][c];
+      }
+    }
+    y[9] = 1.0;
+    for (int i = 8; i >= 0; --i) {
+      double s = 0;
+      for (int j = i + 1; j < 10; ++j) s += M[i][j] * y[j];
+      y[i] = -s / M[i][i];
+    }
+    for (int i = 0; i < 10; ++i) v[cp[i]] = y[i];
+    const int slot = __popc(bal & ((1u << lane) - 1u));
+    for (int k = 0; k < 9; ++k) W.models[slot][k] = E[k][0] * v[6] + E[k][1] * v[7] + E[k][2] * v[8] + E[k][3] * v[9];
+  }
+  if (lane == 0) W.n_models = __popc(bal);
+  __syncwarp();
+}
+
+// FundamentalFromEssential (multiview/essential.cpp:48-53): F = K_J^-T E K_I^-1
+__device__ void fundamental_from_essential(const double *E, const double *intr, double *F) {
+  const double KI[9] = {1.0 / intr[0], 0, -intr[1] / intr[0], 0, 1.0 / intr[0], -intr[2] / intr[0], 0, 0, 1.0};
+  const double KJ[9] = {1.0 / intr[3], 0, -intr[4] / intr[3], 0, 1.0 / intr[3], -intr[5] / intr[3], 0, 0, 1.0};
+  double T[9];
+  for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) { double v = 0; for (int k = 0; k < 3; ++k) v += KJ[3 * k + r] * E[3 * k + c]; T[3 * r + c] = v; }
+  for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) { double v = 0; for (int k = 0; k < 3; ++k) v += T[3 * r + k] * KI[3 * k + c]; F[3 * r + c] = v; }
+}
+
+struct SmemE {                             // the essential instantiation's shared memory (Smem stays the F/H layout)
+  uint32_t mt[624];
+  FivePointWork fp;
+  double Fm[10][9];                         // F in pixels of each real solution (E: fp.models)
+  int hist[NBINS]; int n_le; int warp_cnt[THREADS / 32];
+  uint32_t sample[7];
+  int n_models, better_now;
+  double nfa_thr, nfa_val;
+};
+
+// validation aid: one warp per sample of 5 bearing pairs
+__global__ void __launch_bounds__(32) five_point_kernel(unsigned int n, const double *b1, const double *b2, double *E, int *n_models) {
+  __shared__ FivePointWork W;
+  __shared__ uint32_t sample[5];
+  if (threadIdx.x < 5) sample[threadIdx.x] = threadIdx.x;
+  __syncwarp();
+  for (unsigned int s = blockIdx.x; s < n; s += gridDim.x) {
+    five_point_warp(W, b1 + 15 * (size_t)s, b2 + 15 * (size_t)s, sample, threadIdx.x);
+    for (int e = threadIdx.x; e < 90; e += 32) E[90 * (size_t)s + e] = e / 9 < W.n_models ? W.models[e / 9][e % 9] : 0.0;
+    if (threadIdx.x == 0) n_models[s] = W.n_models;
+    __syncwarp();
+  }
+}
 
 // rand_sampling.hpp:35-58 / 71-95 (thread 0)
 __device__ void sample_reject(Rng &g, int ms, uint32_t total, uint32_t *s) {
@@ -161,25 +514,43 @@ __device__ void sample_shuffle(Rng &g, int ms, uint32_t *vec_index, uint32_t siz
   for (int i = 0; i < ms; ++i) s[i] = vec_index[i];
 }
 
-__global__ void __launch_bounds__(THREADS) acransac_f_kernel(Args A) {
-  __shared__ Smem S;
+// ESSENTIAL = false: the F / H filter (A.model 0 / 1, normalised points, Smem); true: the E filter (five-point solver on
+// bearing vectors, residuals in pixels against F = K_J^-T E K_I^-1, SmemE).
+template <bool ESSENTIAL>
+__global__ void __launch_bounds__(THREADS) acransac_kernel(Args A) {
+  __shared__ typename std::conditional<ESSENTIAL, SmemE, Smem>::type S;
   const double INF = __longlong_as_double(0x7ff0000000000000ll);
   for (unsigned int pair = blockIdx.x; pair < A.n_pairs; pair += gridDim.x) {
     __syncthreads();
     const unsigned long long off = A.offsets[pair];
     const unsigned int nData = (unsigned int)(A.offsets[pair + 1] - off);
     const double *xI = A.xI + 2 * off, *xJ = A.xJ + 2 * off;
-    double *x1 = A.x1 + 2 * off, *x2 = A.x2 + 2 * off;
+    double *x1 = A.x1 + (ESSENTIAL ? 3 : 2) * off, *x2 = A.x2 + (ESSENTIAL ? 3 : 2) * off;   // E: bearing vectors
     uint32_t *vec_index = A.vec_index + off, *inl = A.inliers + off;
     float *logc_n = A.logc_n + off + pair, *logc_k = A.logc_k + off + pair, *l10 = A.l10 + off + pair;
     if (threadIdx.x == 0) {
       A.n_inliers[pair] = 0; A.stats[2 * pair] = 0.0; A.stats[2 * pair + 1] = 0.0;
       for (int i = 0; i < 9; ++i) A.F[9 * (size_t)pair + i] = (i % 4 == 0) ? 1.0 : 0.0;
     }
-    const int ms = A.model == 0 ? 7 : 4;                          // MINIMUM_SAMPLES; MAX_MODELS = 3 / 1
+    const int ms = ESSENTIAL ? 5 : A.model == 0 ? 7 : 4;           // MINIMUM_SAMPLES; MAX_MODELS = 10 / 3 / 1
     if (nData <= (unsigned int)ms) continue;                      // ACRANSAC: nData <= sizeSample -> {0, 0}
     // ---- kernel adaptor: normalisation (conditioning.cpp:54-77), logalpha0
     const int wI = A.image_size[4 * pair], hI = A.image_size[4 * pair + 1], wJ = A.image_size[4 * pair + 2], hJ = A.image_size[4 * pair + 3];
+    double logalpha0, mult_error, maxThreshold;
+    if constexpr (ESSENTIAL) {
+      // ACKernelAdaptorEssential: no normalisation (N1 = N2 = I); bearings = normalize(K^-1 [x; 1]) (Camera_Pinhole.hpp:136-139)
+      const double *k = A.intr + 6 * (size_t)pair;
+      for (unsigned int i = threadIdx.x; i < nData; i += THREADS) {
+        double u = (xI[2 * i] - k[1]) / k[0], v = (xI[2 * i + 1] - k[2]) / k[0], nrm = sqrt(u * u + v * v + 1.0);
+        x1[3 * i] = u / nrm; x1[3 * i + 1] = v / nrm; x1[3 * i + 2] = 1.0 / nrm;
+        u = (xJ[2 * i] - k[4]) / k[3]; v = (xJ[2 * i + 1] - k[5]) / k[3]; nrm = sqrt(u * u + v * v + 1.0);
+        x2[3 * i] = u / nrm; x2[3 * i + 1] = v / nrm; x2[3 * i + 2] = 1.0 / nrm;
+        vec_index[i] = i;
+      }
+      logalpha0 = log10(2. * hypot((double)wJ, (double)hJ) / (wJ * (double)hJ) / 0.5);
+      mult_error = 0.5;
+      maxThreshold = A.precision * A.precision;
+    } else {
     if (threadIdx.x == 0) {
       const double d1 = 1.0 / sqrt((double)(wI * hI)), d2 = 1.0 / sqrt((double)(wJ * hJ));
       for (int i = 0; i < 9; ++i) { S.N1[i] = 0; S.N2[i] = 0; }
@@ -192,10 +563,11 @@ __global__ void __launch_bounds__(THREADS) acransac_f_kernel(Args A) {
       x2[2 * i] = (S.N2[0] * xJ[2 * i] + S.N2[2]) / 1.0; x2[2 * i + 1] = (S.N2[4] * xJ[2 * i + 1] + S.N2[5]) / 1.0;
       vec_index[i] = i;
     }
-    const double logalpha0 = A.model == 0 ? log10(2. * hypot((double)wJ, (double)hJ) / (wJ * (double)hJ) / S.N2[0])       // point to line
-                                          : log10(3.14159265358979323846 / (wJ * (double)hJ) / (S.N2[0] * S.N2[0]));   // point to point
-    const double mult_error = A.model == 0 ? 0.5 : 1.0;
-    const double maxThreshold = A.precision * A.precision * S.N2[0] * S.N2[0];
+    logalpha0 = A.model == 0 ? log10(2. * hypot((double)wJ, (double)hJ) / (wJ * (double)hJ) / S.N2[0])       // point to line
+                             : log10(3.14159265358979323846 / (wJ * (double)hJ) / (S.N2[0] * S.N2[0]));   // point to point
+    mult_error = A.model == 0 ? 0.5 : 1.0;
+    maxThreshold = A.precision * A.precision * S.N2[0] * S.N2[0];
+    }
     // ---- NFA tables (robust_estimator_ACRansac.hpp:57-119), float arithmetic in the reference's order
     for (unsigned int i = threadIdx.x; i <= nData; i += THREADS) l10[i] = (float)log10((double)(float)i);
     __syncthreads();
@@ -207,7 +579,7 @@ __global__ void __launch_bounds__(THREADS) acransac_f_kernel(Args A) {
         if (kk < m) { if (m - kk < kk) kk = m - kk; for (unsigned int i = 1; i <= kk; ++i) r += l10[m - i + 1] - l10[i]; }
         logc_k[k] = r; }
     }
-    const double loge0 = log10((double)(A.model == 0 ? 3 : 1) * (double)(nData - ms));
+    const double loge0 = log10((double)(ESSENTIAL ? 10 : A.model == 0 ? 3 : 1) * (double)(nData - ms));
     __syncthreads();
     // ---- ACRANSAC main loop (robust_estimator_ACRansac.hpp:330-480); the scalars live in every thread (uniform)
     Rng g{S.mt, 624};
@@ -223,6 +595,14 @@ __global__ void __launch_bounds__(THREADS) acransac_f_kernel(Args A) {
         if (bACRansacMode) sample_shuffle(g, ms, vec_index, index_size, S.sample); else sample_reject(g, ms, nData, S.sample);
       }
       __syncthreads();
+      if constexpr (ESSENTIAL) {
+        if (threadIdx.x < 32) {                                   // warp 0: the five-point solver, then F of each model
+          five_point_warp(S.fp, x1, x2, S.sample, threadIdx.x);
+          const int nm = S.fp.n_models;
+          if (threadIdx.x < nm) fundamental_from_essential(S.fp.models[threadIdx.x], A.intr + 6 * (size_t)pair, S.Fm[threadIdx.x]);
+          if (threadIdx.x == 0) S.n_models = nm;
+        }
+      } else {
       // A'A of the 7 epipolar constraints, summed in sample order
       if (threadIdx.x < 81) {
         const int i = threadIdx.x / 9, j = threadIdx.x % 9;
@@ -261,6 +641,7 @@ __global__ void __launch_bounds__(THREADS) acransac_f_kernel(Args A) {
         S.n_models = nr;
         }
       }
+      }
       __syncthreads();
       const int n_models = S.n_models;
       bool better = false;
@@ -272,7 +653,9 @@ __global__ void __launch_bounds__(THREADS) acransac_f_kernel(Args A) {
         const double by_interval = NBINS / (maxThreshold - 0.0);
         int le = 0;
         for (unsigned int i = threadIdx.x; i < nData; i += THREADS) {
-          const double e = model_error(A.model, S.models[mi], x1[2 * i], x1[2 * i + 1], x2[2 * i], x2[2 * i + 1]);
+          double e;
+          if constexpr (ESSENTIAL) e = epipolar_error(S.Fm[mi], xI[2 * i], xI[2 * i + 1], xJ[2 * i], xJ[2 * i + 1]);
+          else e = model_error(A.model, S.models[mi], x1[2 * i], x1[2 * i + 1], x2[2 * i], x2[2 * i + 1]);
           if (e <= maxThreshold) ++le;
           if (e >= 0.0) { const unsigned long long b = (unsigned long long)((e - 0.0) * by_interval); if (b < (unsigned long long)NBINS) atomicAdd(&S.hist[(int)b], 1); }
         }
@@ -304,7 +687,10 @@ __global__ void __launch_bounds__(THREADS) acransac_f_kernel(Args A) {
             for (unsigned int i0 = 0; i0 < nData; i0 += THREADS) {
               const unsigned int i = i0 + threadIdx.x;
               bool in = false;
-              if (i < nData) in = model_error(A.model, S.models[mi], x1[2 * i], x1[2 * i + 1], x2[2 * i], x2[2 * i + 1]) <= thr;
+              if (i < nData) {
+                if constexpr (ESSENTIAL) in = epipolar_error(S.Fm[mi], xI[2 * i], xI[2 * i + 1], xJ[2 * i], xJ[2 * i + 1]) <= thr;
+                else in = model_error(A.model, S.models[mi], x1[2 * i], x1[2 * i + 1], x2[2 * i], x2[2 * i + 1]) <= thr;
+              }
               const unsigned int bal = __ballot_sync(0xffffffffu, in);
               if ((threadIdx.x & 31) == 0) S.warp_cnt[threadIdx.x >> 5] = __popc(bal);
               __syncthreads();
@@ -320,7 +706,10 @@ __global__ void __launch_bounds__(THREADS) acransac_f_kernel(Args A) {
             //  then and the score is NOT updated, robust_estimator_ACRansac.hpp:243-256)
             if (n_inl > (unsigned int)ms) {
               better = true; minNFA = S.nfa_val; errorMax = thr;
-              if (threadIdx.x < 9) A.F[9 * (size_t)pair + threadIdx.x] = S.models[mi][threadIdx.x];
+              if (threadIdx.x < 9) {
+                if constexpr (ESSENTIAL) A.F[9 * (size_t)pair + threadIdx.x] = S.fp.models[mi][threadIdx.x];
+                else A.F[9 * (size_t)pair + threadIdx.x] = S.models[mi][threadIdx.x];
+              }
             }
           }
         }
@@ -340,7 +729,8 @@ __global__ void __launch_bounds__(THREADS) acransac_f_kernel(Args A) {
     if (minNFA >= 0) n_inl = 0;
     if (threadIdx.x == 0) {
       A.n_inliers[pair] = n_inl;
-      if (n_inl > 0) {
+      // E: Unnormalize does nothing and unormalizeError is the identity (errorMax stays squared)
+      if constexpr (!ESSENTIAL) if (n_inl > 0) {
         double M[9], T[9], U[9];
         for (int i = 0; i < 9; ++i) M[i] = A.F[9 * (size_t)pair + i];
         if (A.model == 0) {      // UnnormalizerT: N2' * F * N1
@@ -361,21 +751,31 @@ __global__ void __launch_bounds__(THREADS) acransac_f_kernel(Args A) {
 
 }}  // namespace omvg::geom
 
-extern "C" int omvg_geom_acransac(int device, int32_t model, uint64_t n_pairs, const uint64_t *offsets, const double *xI, const double *xJ,
-                                  const int32_t *image_size, double precision, uint32_t max_iterations,
-                                  uint32_t *inliers, uint32_t *n_inliers, double *F, double *stats) {
+namespace {
+
+// the CUDA device exists and is an sm_90 part; its SM count out
+int check_device(int device, int *n_sms) {
   using namespace omvg;
-  if (model != OMVG_GEOM_FUNDAMENTAL && model != OMVG_GEOM_HOMOGRAPHY) return fail(OMVG_E_UNSUPPORTED, "geometric model %d is not implemented on the GPU path (0 = fundamental, 1 = homography)", model);
+  int n = 0; OMVG_CUDA(cudaGetDeviceCount(&n));
+  if (device < 0 || device >= n) return fail(OMVG_E_CUDA, "no CUDA device %d (found %d)", device, n);
+  int cc_major = 0, cc_minor = 0;
+  OMVG_CUDA(cudaDeviceGetAttribute(&cc_major, cudaDevAttrComputeCapabilityMajor, device));
+  OMVG_CUDA(cudaDeviceGetAttribute(&cc_minor, cudaDevAttrComputeCapabilityMinor, device));
+  OMVG_CUDA(cudaDeviceGetAttribute(n_sms, cudaDevAttrMultiProcessorCount, device));
+  if (cc_major != 9 || cc_minor != 0) return fail(OMVG_E_CUDA, "device %d is sm_%d%d; this library is sm_90a only", device, cc_major, cc_minor);
+  return OMVG_OK;
+}
+
+// everything after the per-model argument checks; intr (model OMVG_GEOM_ESSENTIAL only): [n_pairs][6]
+int geom_run(int device, int32_t model, uint64_t n_pairs, const uint64_t *offsets, const double *xI, const double *xJ,
+             const int32_t *image_size, const double *intr, double precision, uint32_t max_iterations,
+             uint32_t *inliers, uint32_t *n_inliers, double *F, double *stats) {
+  using namespace omvg;
   if (n_pairs && (!offsets || !image_size || !n_inliers || !F || !stats)) return fail(OMVG_E_ARG, "null argument");
   if (!(precision > 0.0) || !std::isfinite(precision)) return fail(OMVG_E_UNSUPPORTED, "the GPU filter needs a finite upper bound of the precision (main_GeometricFilter uses 4.0)");
   if (max_iterations < 1) return fail(OMVG_E_ARG, "max_iterations must be >= 1");
-  int n = 0; OMVG_CUDA(cudaGetDeviceCount(&n));
-  if (device < 0 || device >= n) return fail(OMVG_E_CUDA, "no CUDA device %d (found %d)", device, n);
-  int cc_major = 0, cc_minor = 0, n_sms = 0;
-  OMVG_CUDA(cudaDeviceGetAttribute(&cc_major, cudaDevAttrComputeCapabilityMajor, device));
-  OMVG_CUDA(cudaDeviceGetAttribute(&cc_minor, cudaDevAttrComputeCapabilityMinor, device));
-  OMVG_CUDA(cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, device));
-  if (cc_major != 9 || cc_minor != 0) return fail(OMVG_E_CUDA, "device %d is sm_%d%d; this library is sm_90a only", device, cc_major, cc_minor);
+  int n_sms = 0;
+  if (const int rc = check_device(device, &n_sms)) return rc;
   if (!n_pairs) return OMVG_OK;
   for (uint64_t p = 0; p < n_pairs; ++p) {
     if (offsets[p + 1] < offsets[p]) return fail(OMVG_E_ARG, "offsets must be non-decreasing");
@@ -384,34 +784,80 @@ extern "C" int omvg_geom_acransac(int device, int32_t model, uint64_t n_pairs, c
   const uint64_t nm = offsets[n_pairs];
   if (nm && (!xI || !xJ || !inliers)) return fail(OMVG_E_ARG, "null match arrays");
   if (nm >= (1ull << 31)) return fail(OMVG_E_UNSUPPORTED, "more than 2^31 putative matches in one call");
+  const bool essential = model == OMVG_GEOM_ESSENTIAL;
+  const size_t xs = essential ? 24 : 16;                  // scratch per match: bearing vectors (E) or normalised points
   OMVG_CUDA(cudaSetDevice(device));
   cudaStream_t st; OMVG_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   struct Bufs { std::vector<void *> p; cudaStream_t s; ~Bufs() { for (void *q : p) pool_free(q); cudaStreamDestroy(s); } } B{{}, st};
   auto dalloc = [&](size_t bytes) -> void * { void *q = nullptr; if (pool_malloc(&q, std::max<size_t>(bytes, 8)) != cudaSuccess) return nullptr; B.p.push_back(q); return q; };
   geom::Args A{};
   unsigned long long *d_off = (unsigned long long *)dalloc((n_pairs + 1) * 8);
-  double *d_xI = (double *)dalloc(nm * 16), *d_xJ = (double *)dalloc(nm * 16), *d_x1 = (double *)dalloc(nm * 16), *d_x2 = (double *)dalloc(nm * 16);
+  double *d_xI = (double *)dalloc(nm * 16), *d_xJ = (double *)dalloc(nm * 16), *d_x1 = (double *)dalloc(nm * xs), *d_x2 = (double *)dalloc(nm * xs);
   int *d_sz = (int *)dalloc(n_pairs * 16);
   float *d_ln = (float *)dalloc((nm + n_pairs) * 4), *d_lk = (float *)dalloc((nm + n_pairs) * 4), *d_l10 = (float *)dalloc((nm + n_pairs) * 4);
   uint32_t *d_idx = (uint32_t *)dalloc(nm * 4), *d_inl = (uint32_t *)dalloc(nm * 4), *d_ninl = (uint32_t *)dalloc(n_pairs * 4);
   double *d_F = (double *)dalloc(n_pairs * 72), *d_stats = (double *)dalloc(n_pairs * 16);
-  if (!d_off || !d_xI || !d_xJ || !d_x1 || !d_x2 || !d_sz || !d_ln || !d_lk || !d_l10 || !d_idx || !d_inl || !d_ninl || !d_F || !d_stats) return fail(OMVG_E_CUDA, "out of device memory");
+  double *d_intr = essential ? (double *)dalloc(n_pairs * 48) : nullptr;
+  if (!d_off || !d_xI || !d_xJ || !d_x1 || !d_x2 || !d_sz || !d_ln || !d_lk || !d_l10 || !d_idx || !d_inl || !d_ninl || !d_F || !d_stats || (essential && !d_intr)) return fail(OMVG_E_CUDA, "out of device memory");
+  if (essential) OMVG_CUDA(cudaMemcpyAsync(d_intr, intr, n_pairs * 48, cudaMemcpyHostToDevice, st));
   OMVG_CUDA(cudaMemcpyAsync(d_off, offsets, (n_pairs + 1) * 8, cudaMemcpyHostToDevice, st));
   OMVG_CUDA(cudaMemcpyAsync(d_sz, image_size, n_pairs * 16, cudaMemcpyHostToDevice, st));
   if (nm) { OMVG_CUDA(cudaMemcpyAsync(d_xI, xI, nm * 16, cudaMemcpyHostToDevice, st)); OMVG_CUDA(cudaMemcpyAsync(d_xJ, xJ, nm * 16, cudaMemcpyHostToDevice, st)); }
   A.model = model;
   A.offsets = d_off; A.xI = d_xI; A.xJ = d_xJ; A.image_size = d_sz; A.precision = precision; A.iterations = max_iterations;
   A.x1 = d_x1; A.x2 = d_x2; A.logc_n = d_ln; A.logc_k = d_lk; A.l10 = d_l10; A.vec_index = d_idx; A.inliers = d_inl; A.n_inliers = d_ninl; A.F = d_F; A.stats = d_stats;
-  A.n_pairs = (unsigned int)n_pairs;
-  int per_sm = 1; OMVG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, geom::acransac_f_kernel, geom::THREADS, 0));
+  A.n_pairs = (unsigned int)n_pairs; A.intr = d_intr;
+  void (*kernel)(geom::Args) = essential ? geom::acransac_kernel<true> : geom::acransac_kernel<false>;
+  int per_sm = 1; OMVG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, geom::THREADS, 0));
   const unsigned int grid = (unsigned int)std::min<uint64_t>(n_pairs, (uint64_t)n_sms * std::max(1, per_sm));
-  geom::acransac_f_kernel<<<grid, geom::THREADS, 0, st>>>(A);
+  kernel<<<grid, geom::THREADS, 0, st>>>(A);
   OMVG_CUDA(cudaGetLastError());
   if (nm) OMVG_CUDA(cudaMemcpyAsync(inliers, d_inl, nm * 4, cudaMemcpyDeviceToHost, st));
   OMVG_CUDA(cudaMemcpyAsync(n_inliers, d_ninl, n_pairs * 4, cudaMemcpyDeviceToHost, st));
   OMVG_CUDA(cudaMemcpyAsync(F, d_F, n_pairs * 72, cudaMemcpyDeviceToHost, st));
   OMVG_CUDA(cudaMemcpyAsync(stats, d_stats, n_pairs * 16, cudaMemcpyDeviceToHost, st));
   OMVG_CUDA(cudaStreamSynchronize(st));
+  return OMVG_OK;
+}
+
+}  // namespace
+
+extern "C" int omvg_geom_acransac(int device, int32_t model, uint64_t n_pairs, const uint64_t *offsets, const double *xI, const double *xJ,
+                                  const int32_t *image_size, double precision, uint32_t max_iterations,
+                                  uint32_t *inliers, uint32_t *n_inliers, double *F, double *stats) {
+  using namespace omvg;
+  if (model != OMVG_GEOM_FUNDAMENTAL && model != OMVG_GEOM_HOMOGRAPHY) return fail(OMVG_E_UNSUPPORTED, "geometric model %d is not implemented on the GPU path (0 = fundamental, 1 = homography; the essential model needs intrinsics: omvg_geom_essential_acransac)", model);
+  return geom_run(device, model, n_pairs, offsets, xI, xJ, image_size, nullptr, precision, max_iterations, inliers, n_inliers, F, stats);
+}
+
+extern "C" int omvg_geom_essential_acransac(int device, uint64_t n_pairs, const uint64_t *offsets, const double *xI, const double *xJ,
+                                            const int32_t *image_size, const double *intr, double precision, uint32_t max_iterations,
+                                            uint32_t *inliers, uint32_t *n_inliers, double *E, double *stats) {
+  using namespace omvg;
+  if (n_pairs && !intr) return fail(OMVG_E_ARG, "null intrinsics");
+  for (uint64_t p = 0; p < n_pairs; ++p) {
+    const double *k = intr + 6 * p;
+    if (!(k[0] > 0.0) || !(k[3] > 0.0) || !std::isfinite(k[0]) || !std::isfinite(k[3])) return fail(OMVG_E_ARG, "pair %llu: the focal lengths must be finite and > 0", (unsigned long long)p);
+    if (!std::isfinite(k[1]) || !std::isfinite(k[2]) || !std::isfinite(k[4]) || !std::isfinite(k[5])) return fail(OMVG_E_ARG, "pair %llu: non-finite principal point", (unsigned long long)p);
+  }
+  return geom_run(device, OMVG_GEOM_ESSENTIAL, n_pairs, offsets, xI, xJ, image_size, intr, precision, max_iterations, inliers, n_inliers, E, stats);
+}
+
+extern "C" int omvg_geom_debug_five_point(int device, uint32_t n, const double *b1, const double *b2, double *E, int32_t *n_models) {
+  using namespace omvg;
+  if (n && (!b1 || !b2 || !E || !n_models)) return fail(OMVG_E_ARG, "null argument");
+  int n_sms = 0;
+  if (const int rc = check_device(device, &n_sms)) return rc;
+  if (!n) return OMVG_OK;
+  OMVG_CUDA(cudaSetDevice(device));
+  double *d_b1 = nullptr, *d_b2 = nullptr, *d_E = nullptr; int *d_n = nullptr;
+  struct Bufs { void **p[4]; ~Bufs() { for (void **q : p) if (*q) cudaFree(*q); } } B{{(void **)&d_b1, (void **)&d_b2, (void **)&d_E, (void **)&d_n}};
+  OMVG_CUDA(cudaMalloc(&d_b1, n * 120ull)); OMVG_CUDA(cudaMalloc(&d_b2, n * 120ull));
+  OMVG_CUDA(cudaMalloc(&d_E, n * 720ull)); OMVG_CUDA(cudaMalloc(&d_n, n * 4ull));
+  OMVG_CUDA(cudaMemcpy(d_b1, b1, n * 120ull, cudaMemcpyHostToDevice)); OMVG_CUDA(cudaMemcpy(d_b2, b2, n * 120ull, cudaMemcpyHostToDevice));
+  geom::five_point_kernel<<<std::min<uint32_t>(n, 64u * n_sms), 32>>>(n, d_b1, d_b2, d_E, d_n);
+  OMVG_CUDA(cudaGetLastError());
+  OMVG_CUDA(cudaMemcpy(E, d_E, n * 720ull, cudaMemcpyDeviceToHost)); OMVG_CUDA(cudaMemcpy(n_models, d_n, n * 4ull, cudaMemcpyDeviceToHost));
   return OMVG_OK;
 }
 

@@ -13,7 +13,7 @@ from ._lib import check, lib
 _vp = ctypes.c_void_p
 
 
-FUNDAMENTAL, HOMOGRAPHY = 0, 1
+FUNDAMENTAL, HOMOGRAPHY, ESSENTIAL = 0, 1, 2
 
 
 def fundamental_acransac(offsets, xI, xJ, image_size, precision: float = 4.0, max_iterations: int = 2048, device: int = 0):
@@ -41,3 +41,35 @@ def acransac(model, offsets, xI, xJ, image_size, precision: float = 4.0, max_ite
         a = int(off[k])
         out.append(dict(inliers=inl[a:a + int(ninl[k])].copy(), F=F[k].reshape(3, 3).copy(), error_max=float(st[k, 0]), min_nfa=float(st[k, 1])))
     return out
+
+
+def essential_acransac(offsets, xI, xJ, image_size, intr, precision: float = 4.0, max_iterations: int = 2048, device: int = 0):
+    """GeometricFilter_EMatrix_AC::Robust_estimation per pair (E_ACRobust.hpp:55-150) over a CSR of putative matches of
+    calibrated pinhole views.  intr [n_pairs, 6] = (f, ppx, ppy) of view I then view J.  Same result dicts as
+    acransac; `F` holds E and error_max is in squared pixels, as the reference leaves them.  The reference keeps a
+    pair iff it has more than 12.5 inliers."""
+    off = np.ascontiguousarray(offsets, np.uint64); n_pairs = len(off) - 1
+    xI = np.ascontiguousarray(xI, np.float64).reshape(-1, 2); xJ = np.ascontiguousarray(xJ, np.float64).reshape(-1, 2)
+    sz = np.ascontiguousarray(image_size, np.int32).reshape(-1, 4)
+    k = np.ascontiguousarray(intr, np.float64).reshape(-1, 6)
+    nm = int(off[-1]); assert len(xI) == nm == len(xJ) and len(sz) == n_pairs == len(k)
+    inl = np.zeros(max(nm, 1), np.uint32); ninl = np.zeros(max(n_pairs, 1), np.uint32); E = np.zeros((max(n_pairs, 1), 9)); st = np.zeros((max(n_pairs, 1), 2))
+    p = lambda a: a.ctypes.data_as(_vp)   # noqa: E731
+    check(lib().omvg_geom_essential_acransac(int(device), ctypes.c_uint64(n_pairs), p(off), p(xI), p(xJ), p(sz), p(k), ctypes.c_double(precision),
+                                             ctypes.c_uint32(max_iterations), p(inl), p(ninl), p(E), p(st)))
+    out = []
+    for q in range(n_pairs):
+        a = int(off[q])
+        out.append(dict(inliers=inl[a:a + int(ninl[q])].copy(), F=E[q].reshape(3, 3).copy(), error_max=float(st[q, 0]), min_nfa=float(st[q, 1])))
+    return out
+
+
+def debug_five_point(b1, b2, device: int = 0):
+    """The device five-point solver on n samples of 5 bearing pairs [n, 5, 3] (validation aid).
+    -> dict(E [n, 10, 3, 3], n_models [n]): the first n_models[s] matrices of sample s are its real solutions."""
+    b1 = np.ascontiguousarray(b1, np.float64).reshape(-1, 5, 3); b2 = np.ascontiguousarray(b2, np.float64).reshape(-1, 5, 3)
+    n = len(b1); assert len(b2) == n
+    E = np.zeros((max(n, 1), 10, 9)); k = np.zeros(max(n, 1), np.int32)
+    p = lambda a: a.ctypes.data_as(_vp)   # noqa: E731
+    check(lib().omvg_geom_debug_five_point(int(device), ctypes.c_uint32(n), p(b1), p(b2), p(E), p(k)))
+    return dict(E=E[:n].reshape(n, 10, 3, 3).copy(), n_models=k[:n].copy())

@@ -9,10 +9,15 @@
 // pair is kept iff it has more than 2.5 * 7 inliers (F_ACRobust.hpp:85).  Guided matching is not part of this path.
 //
 // Robust_model_estimation_H is the same for GeometricFilter_HMatrix_AC (H_ACRobust.hpp: 4-point homography).
+// Robust_model_estimation_E is GeometricFilter_EMatrix_AC (E_ACRobust.hpp:55-150: five-point essential matrix of calibrated
+// views): pairs whose views lack an intrinsic or have a non-pinhole one are skipped and not kept, as the reference skips
+// them; K comes from Pinhole_Intrinsic::K(); the pair is kept iff it has more than 2.5 * 5 inliers.
 // Header-only; compile inside an openMVG build and link libomvg_b200.so.
 #ifndef OPENMVG_B200_GEOMETRIC_FILTER_B200_HPP
 #define OPENMVG_B200_GEOMETRIC_FILTER_B200_HPP
 
+#include "openMVG/cameras/Camera_Common.hpp"
+#include "openMVG/cameras/Camera_Pinhole.hpp"
 #include "openMVG/matching/indMatch.hpp"
 #include "openMVG/matching_image_collection/Geometric_Filter_utils.hpp"
 #include "openMVG/sfm/pipelines/sfm_regions_provider.hpp"
@@ -41,6 +46,10 @@ struct ImageCollectionGeometricFilter_B200
   bool Robust_model_estimation_H(const matching::PairWiseMatches & putative_matches, double dPrecision = 4.0, uint32_t iteration = 2048,
                                  system::ProgressInterface * my_progress_bar = nullptr)
   { return Robust_model_estimation(OMVG_GEOM_HOMOGRAPHY, putative_matches, dPrecision, iteration, my_progress_bar); }
+  // E model (GeometricFilter_EMatrix_AC(dPrecision, iteration), E_ACRobust.hpp:55-150): kept iff more than 2.5 * 5 inliers
+  bool Robust_model_estimation_E(const matching::PairWiseMatches & putative_matches, double dPrecision = 4.0, uint32_t iteration = 2048,
+                                 system::ProgressInterface * my_progress_bar = nullptr)
+  { return Robust_model_estimation(OMVG_GEOM_ESSENTIAL, putative_matches, dPrecision, iteration, my_progress_bar); }
 
   bool Robust_model_estimation(int32_t model, const matching::PairWiseMatches & putative_matches, double dPrecision, uint32_t iteration,
                                system::ProgressInterface * my_progress_bar = nullptr)
@@ -50,9 +59,32 @@ struct ImageCollectionGeometricFilter_B200
     std::vector<uint64_t> offsets(1, 0);
     std::vector<double> xI, xJ;
     std::vector<int32_t> size;
+    std::vector<double> intr;                                   // E: f, ppx, ppy of view I then view J, per pair sent
     std::vector<const std::pair<const Pair, matching::IndMatches> *> order;
+    const bool essential = model == OMVG_GEOM_ESSENTIAL;
+    size_t skipped = 0;
     for (const auto & it : putative_matches)
     {
+      if (essential)                                            // E_ACRobust.hpp:74-98
+      {
+        const cameras::IntrinsicBase * cam[2] = {nullptr, nullptr};
+        const IndexT ids[2] = {it.first.first, it.first.second};
+        for (int k = 0; k < 2; ++k)
+        {
+          const IndexT id_intrinsic = sfm_data_->views.at(ids[k])->id_intrinsic;
+          if (sfm_data_->GetIntrinsics().count(id_intrinsic)) cam[k] = sfm_data_->GetIntrinsics().at(id_intrinsic).get();
+        }
+        if (!cam[0] || !cam[1] || !cameras::isPinhole(cam[0]->getType()) || !cameras::isPinhole(cam[1]->getType()))
+        {
+          ++skipped;
+          continue;
+        }
+        for (int k = 0; k < 2; ++k)
+        {
+          const Mat3 & K = dynamic_cast<const cameras::Pinhole_Intrinsic *>(cam[k])->K();
+          intr.insert(intr.end(), {K(0, 0), K(0, 2), K(1, 2)});
+        }
+      }
       Mat2X a, b;
       MatchesPairToMat(it.first, it.second, sfm_data_, regions_provider_, a, b);
       for (Mat2X::Index k = 0; k < a.cols(); ++k) { xI.push_back(a(0, k)); xI.push_back(a(1, k)); xJ.push_back(b(0, k)); xJ.push_back(b(1, k)); }
@@ -65,16 +97,21 @@ struct ImageCollectionGeometricFilter_B200
     std::vector<uint32_t> inliers(xI.size() / 2 + 1), n_inliers(n_pairs + 1);
     F_.assign(9 * n_pairs, 0.0); stats_.assign(2 * n_pairs, 0.0);
     _map_GeometricMatches.clear();
-    const double min_samples = model == OMVG_GEOM_FUNDAMENTAL ? 7.0 : 4.0;
-    if (omvg_geom_acransac(device_, model, n_pairs, offsets.data(), xI.data(), xJ.data(), size.data(), dPrecision, iteration,
-                                       inliers.data(), n_inliers.data(), F_.data(), stats_.data()) != OMVG_OK)
+    const double min_samples = model == OMVG_GEOM_FUNDAMENTAL ? 7.0 : essential ? 5.0 : 4.0;
+    const int rc = essential
+      ? omvg_geom_essential_acransac(device_, n_pairs, offsets.data(), xI.data(), xJ.data(), size.data(), intr.data(), dPrecision, iteration,
+                                     inliers.data(), n_inliers.data(), F_.data(), stats_.data())
+      : omvg_geom_acransac(device_, model, n_pairs, offsets.data(), xI.data(), xJ.data(), size.data(), dPrecision, iteration,
+                           inliers.data(), n_inliers.data(), F_.data(), stats_.data());
+    for (size_t p = 0; p < skipped; ++p) ++(*my_progress_bar);
+    if (rc != OMVG_OK)
     {
       OPENMVG_LOG_ERROR << "omvg_b200: " << omvg_last_error();
       return false;
     }
     for (size_t p = 0; p < n_pairs; ++p)
     {
-      if (n_inliers[p] > min_samples * 2.5)                      // F_ACRobust.hpp:85, H_ACRobust.hpp:97
+      if (n_inliers[p] > min_samples * 2.5)                      // F_ACRobust.hpp:85, H_ACRobust.hpp:97, E_ACRobust.hpp:135
       {
         matching::IndMatches geometric_inliers;
         geometric_inliers.reserve(n_inliers[p]);
@@ -92,7 +129,7 @@ struct ImageCollectionGeometricFilter_B200
   const std::shared_ptr<sfm::Regions_Provider> regions_provider_;   // (a copy: the reference keeps a reference, which dangles when bound to a converted temporary)
   int device_;
   matching::PairWiseMatches _map_GeometricMatches;
-  std::vector<double> F_, stats_;                               // per pair (map order): un-normalised F, {errorMax, minNFA}
+  std::vector<double> F_, stats_;                               // per pair sent (map order): un-normalised F (H, E), {errorMax, minNFA}
 };
 
 }  // namespace matching_image_collection

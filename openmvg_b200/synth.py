@@ -265,3 +265,35 @@ def two_view_matches(n: int, outlier_frac: float = 0.3, noise_px: float = 0.5, s
     out = rng.random(n) < outlier_frac
     xJ[out] = np.stack([rng.uniform(0, w, int(out.sum())), rng.uniform(0, h, int(out.sum()))], 1)
     return xI.astype(np.float32).astype(np.float64), xJ.astype(np.float32).astype(np.float64), ~out
+
+
+def calibrated_two_view_matches(n: int, outlier_frac: float = 0.3, seed: int = 3, wh=(1600, 1200), intr_I=None, intr_J=None,
+                                noise_px: float = 0.5, motion: str = "general"):
+    """Putative matches of one CALIBRATED image pair for the essential-matrix filter (DESIGN §3.8): like
+    two_view_matches, but each view has its own pinhole intrinsic (f, ppx, ppy), by default with different focal
+    lengths and principal points.  motion: "general" (sideways + rotation), "short" (a baseline of 2 % of the depth),
+    "forward" (the camera moves along its optical axis), "planar" (the points lie close to a plane).
+    -> (xI [n,2], xJ [n,2]) float64, inlier mask [n], intr_I (f, ppx, ppy), intr_J (f, ppx, ppy)"""
+    rng = np.random.default_rng(seed)
+    w, h = wh
+    if intr_I is None:
+        intr_I = (1.1 * max(w, h), w / 2 + 13.5, h / 2 - 7.25)
+    if intr_J is None:
+        intr_J = (0.9 * max(w, h), w / 2 - 21.0, h / 2 + 9.5)
+    X = np.stack([rng.uniform(-1.5, 1.5, n), rng.uniform(-1.2, 1.2, n), rng.uniform(4.0, 9.0, n)], 1)
+    if motion == "planar":
+        X[:, 2] = 6.0 + 0.3 * X[:, 0] - 0.2 * X[:, 1] + rng.normal(0, 0.01, n)
+    R2, C2 = {"general": (_rodrigues(np.array([0.03, -0.25, 0.02])), np.array([1.2, 0.05, 0.3])),
+              "short": (_rodrigues(np.array([0.01, -0.02, 0.005])), np.array([0.12, 0.01, 0.02])),
+              "forward": (_rodrigues(np.array([0.01, 0.02, -0.01])), np.array([0.02, -0.01, 1.5])),
+              "planar": (_rodrigues(np.array([0.05, -0.2, 0.03])), np.array([1.0, 0.1, 0.2]))}[motion]
+
+    def proj(R, C, k):
+        Xc = (X - C) @ R.T
+        return np.stack([k[1] + k[0] * Xc[:, 0] / Xc[:, 2], k[2] + k[0] * Xc[:, 1] / Xc[:, 2]], 1)
+    xI = proj(np.eye(3), np.zeros(3), intr_I) + rng.normal(0, noise_px, (n, 2))
+    xJ = proj(R2, C2, intr_J) + rng.normal(0, noise_px, (n, 2))
+    out = rng.random(n) < outlier_frac
+    xJ[out] = np.stack([rng.uniform(0, w, int(out.sum())), rng.uniform(0, h, int(out.sum()))], 1)
+    return (xI.astype(np.float32).astype(np.float64), xJ.astype(np.float32).astype(np.float64), ~out,
+            tuple(float(v) for v in intr_I), tuple(float(v) for v in intr_J))
