@@ -73,8 +73,10 @@ struct omvg_ba_ctx {
   DevBuf<double> part, part2, part3, icol_part, scal;
   DevBuf<int> fail;
   DevBuf<unsigned long long> pcg_tim;
-  DevBuf<double> corner_rep;
-  DevBuf<double> H;                         // per observation L^-1 E'Fc (schur_stage_kernel -> schur_gather_kernel)
+  DevBuf<double> H;                         // per observation L^-1 E'Fc (schur_stage_kernel -> schur_gather_kernel, schur_border_kernel)
+  DevBuf<double> Gv;                        // per landmark {L^-1 E'b, L^-1 E'Fi} (schur_stage_kernel -> schur_border_kernel, corner_kernel)
+  DevBuf<int> cam_seg, seg_start, seg_intr; int nseg = 0;   // (pose, intrinsic group) segments of the per-pose lists
+  DevBuf<double> FiFc, corner_part; int corner_chunks = 1;   // per segment Fi'Fc (cam_colsum_kernel); corner partial sums
   DevBuf<int2> pair; DevBuf<int> pair_start, chunk_blk, chunk_first, ticket; DevBuf<double> gpart; int n_chunks = 0;   // co-visibility lists (schur_gather_kernel)
   // optional extensions: GCP weights / flags / fixed landmarks, pose-centre priors
   DevBuf<double> obs_w; DevBuf<unsigned char> obs_flags, pt_fixed; DevBuf<unsigned> pt_mask;
@@ -176,7 +178,10 @@ int eval_cost(omvg_ba_ctx *c, const omvg_ba_options *o, int which, int slot) {
 
 int colsums(omvg_ba_ctx *c) {
   point_accum_kernel<<<(c->np + 127) / 128, 128, 0, c->stream>>>(c->Jp.p, c->Ji.p, c->r.p, c->pt_start.p, c->pt_single.p, c->np, c->no, c->kiu, c->EtE.p, c->Etb.p, c->EtFi.p, c->diag_pt.p); LAUNCH_CHECK();
-  cam_colsum_kernel<<<c->nc, CCS_THREADS, 0, c->stream>>>(c->Jc.p, c->r.p, c->cam_start.p, c->cam_obs.p, c->nc, c->no, c->diag_cam.p, c->g_cam.p, c->FtF.p); LAUNCH_CHECK();
+#define CCS(K) cam_colsum_kernel<K><<<c->nc, CCS_THREADS, 0, c->stream>>>(c->Jc.p, c->Ji.p, c->r.p, c->cam_seg.p, c->seg_start.p, c->cam_obs.p, c->nc, c->no, c->diag_cam.p, c->g_cam.p, c->FtF.p, c->FiFc.p)
+  switch (c->kiu) { case 3: CCS(3); break; case 4: CCS(4); break; case 6: CCS(6); break; case 7: CCS(7); break; default: CCS(8); break; }
+#undef CCS
+  LAUNCH_CHECK();
   if (c->npri) { prior_accum_kernel<<<(c->npri + 127) / 128, 128, 0, c->stream>>>(c->JP.p, c->rP.p, c->prior_pose.p, c->npri, c->diag_cam.p, c->g_cam.p, c->FtF.p); LAUNCH_CHECK(); c->launches++; }
   const int chunks = c->ics_chunks;
   { const dim3 g(chunks, c->ni);
@@ -495,7 +500,7 @@ int omvg_ba_create(omvg_ba_ctx **out, int device, const omvg_ba_problem *P) {
   // the image positions / weights / flags (16-25 B per observation) are only needed by the last gather: their upload runs on
   // a second stream under the sorts and the structure build (pinned host buffers; pageable ones are staged synchronously)
   DevBuf<double> raw_xy, raw_w; DevBuf<unsigned char> raw_fl;
-  { DevBuf<int> raw_view, raw_point, d_view_pose, d_view_intr, keys, iota, keys2, bad; DevBuf<unsigned char> cubtmp;
+  { DevBuf<int> raw_view, raw_point, d_view_pose, d_view_intr, keys, iota, keys2, bad, perm1, flag, seg_id; DevBuf<unsigned char> cubtmp;
     UP(raw_view, P->obs_view, no); UP(raw_point, P->obs_point, no);
     UP(d_view_pose, P->view_pose, c->nv); UP(d_view_intr, P->view_intr, c->nv);
     if ((rc = upload(raw_xy, P->obs_xy, (size_t)(2 * no), c->stream2))) return rc;
@@ -504,7 +509,8 @@ int omvg_ba_create(omvg_ba_ctx **out, int device, const omvg_ba_problem *P) {
     OMVG_CUDA(cudaEventRecord(c->ev_up, c->stream2));
     if (tm.on) { cudaStreamSynchronize(s); cudaStreamSynchronize(c->stream2); }
     tm.lap("uploads");
-    if ((rc = keys.alloc(no)) || (rc = iota.alloc(no)) || (rc = keys2.alloc(no)) || (rc = bad.alloc(1))) return rc;
+    if ((rc = keys.alloc(no)) || (rc = iota.alloc(no)) || (rc = keys2.alloc(no)) || (rc = bad.alloc(1)) || (rc = flag.alloc(no + 1)) || (rc = seg_id.alloc(no + 1))) return rc;
+    if (c->ni > 1 && (rc = perm1.alloc(no))) return rc;
     if ((rc = c->d_perm.alloc(no)) || (rc = c->obs_pose.alloc(no)) || (rc = c->obs_intr.alloc(no)) || (rc = c->obs_pt.alloc(no)) || (rc = c->obs_xy.alloc(2 * no))) return rc;
     if ((rc = c->pt_start.alloc(c->np + 1)) || (rc = c->cam_start.alloc(c->nc + 1)) || (rc = c->cam_obs.alloc(no)) || (rc = c->pt_single.alloc(c->np))) return rc;
     const int h_big = 0x7fffffff; OMVG_CUDA(cudaMemcpyAsync(bad.p, &h_big, sizeof(int), cudaMemcpyHostToDevice, s));
@@ -512,26 +518,46 @@ int omvg_ba_create(omvg_ba_ctx **out, int device, const omvg_ba_problem *P) {
     setup_check_kernel<<<gb, 256, 0, s>>>(raw_view.p, raw_point.p, no, c->nv, c->np, keys.p, iota.p, bad.p); LAUNCH_CHECK();
     int pbits = 1; while ((1ll << pbits) < c->np) ++pbits;
     int cbits = 1; while ((1ll << cbits) < c->nc) ++cbits;
-    size_t tb1 = 0, tb2 = 0;                                  // stable LSD radix sorts (CUB): by landmark, then by pose
+    int ibits = 1; while ((1ll << ibits) < c->ni) ++ibits;
+    size_t tb1 = 0, tb2 = 0, tb3 = 0, tb4 = 0;                // stable LSD radix sorts (CUB): by landmark, then by pose
     OMVG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb1, keys.p, c->obs_pt.p, iota.p, c->d_perm.p, (int)no, 0, pbits, s));
     OMVG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb2, c->obs_pose.p, keys2.p, iota.p, c->cam_obs.p, (int)no, 0, cbits, s));
-    if ((rc = cubtmp.alloc(std::max(tb1, tb2)))) return rc;
+    OMVG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb3, c->obs_intr.p, keys.p, iota.p, perm1.p, (int)no, 0, ibits, s));
+    OMVG_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb4, flag.p, seg_id.p, no + 1, s));
+    if ((rc = cubtmp.alloc(std::max(std::max(tb1, tb2), std::max(tb3, tb4))))) return rc;
     size_t tb = cubtmp.n;
     OMVG_CUDA(cub::DeviceRadixSort::SortPairs(cubtmp.p, tb, keys.p, c->obs_pt.p, iota.p, c->d_perm.p, (int)no, 0, pbits, s));
     setup_gather_kernel<<<gb, 256, 0, s>>>(c->d_perm.p, raw_view.p, d_view_pose.p, d_view_intr.p, nullptr, nullptr, nullptr, no, c->nv,
                                            c->obs_pose.p, c->obs_intr.p, nullptr, nullptr, nullptr, iota.p); LAUNCH_CHECK();
     setup_starts_kernel<<<(unsigned)((no + 256) / 256), 256, 0, s>>>(c->obs_pt.p, no, c->np, c->pt_start.p); LAUNCH_CHECK();
+    // the per-pose lists: landmark order within each intrinsic group of the pose (with several groups a stable sort by
+    // group comes first), cut into (pose, group) segments: the blocks of the intrinsics border
+    const int *pose_key = c->obs_pose.p, *pose_val = iota.p;
+    if (c->ni > 1) {
+      tb = cubtmp.n;
+      OMVG_CUDA(cub::DeviceRadixSort::SortPairs(cubtmp.p, tb, c->obs_intr.p, keys.p, iota.p, perm1.p, (int)no, 0, ibits, s));
+      setup_permute_kernel<<<gb, 256, 0, s>>>(perm1.p, c->obs_pose.p, no, keys.p); LAUNCH_CHECK();
+      pose_key = keys.p; pose_val = perm1.p; c->launches++;
+    }
     tb = cubtmp.n;
-    OMVG_CUDA(cub::DeviceRadixSort::SortPairs(cubtmp.p, tb, c->obs_pose.p, keys2.p, iota.p, c->cam_obs.p, (int)no, 0, cbits, s));
+    OMVG_CUDA(cub::DeviceRadixSort::SortPairs(cubtmp.p, tb, pose_key, keys2.p, pose_val, c->cam_obs.p, (int)no, 0, cbits, s));
     setup_starts_kernel<<<(unsigned)((no + 256) / 256), 256, 0, s>>>(keys2.p, no, c->nc, c->cam_start.p); LAUNCH_CHECK();
+    setup_seg_flag_kernel<<<(unsigned)((no + 256) / 256), 256, 0, s>>>(keys2.p, c->cam_obs.p, c->obs_intr.p, no, flag.p); LAUNCH_CHECK();
+    tb = cubtmp.n;
+    OMVG_CUDA(cub::DeviceScan::ExclusiveSum(cubtmp.p, tb, flag.p, seg_id.p, no + 1, s));
     DevBuf<int> slow; if ((rc = slow.alloc(1))) return rc;
     OMVG_CUDA(cudaMemsetAsync(slow.p, 0, sizeof(int), s));
     setup_single_kernel<<<(c->np + 255) / 256, 256, 0, s>>>(c->obs_intr.p, c->pt_start.p, c->np, c->pt_single.p, slow.p); LAUNCH_CHECK();
     int h_bad = 0; OMVG_CUDA(cudaMemcpyAsync(&h_bad, bad.p, sizeof(int), cudaMemcpyDeviceToHost, s));
     OMVG_CUDA(cudaMemcpyAsync(&c->n_slow, slow.p, sizeof(int), cudaMemcpyDeviceToHost, s));
-    OMVG_CUDA(cudaStreamSynchronize(s));                      // the temporaries above are released at the end of this scope
-    c->launches += 9;
+    OMVG_CUDA(cudaMemcpyAsync(&c->nseg, seg_id.p + no, sizeof(int), cudaMemcpyDeviceToHost, s));
+    OMVG_CUDA(cudaStreamSynchronize(s));
     if (h_bad != h_big) return fail(OMVG_E_ARG, "observation %d out of range", h_bad);
+    if ((rc = c->seg_start.alloc(c->nseg + 1)) || (rc = c->seg_intr.alloc(c->nseg)) || (rc = c->cam_seg.alloc(c->nc + 1))) return rc;
+    setup_seg_emit_kernel<<<(unsigned)((std::max<long long>(no, c->nc) + 256) / 256), 256, 0, s>>>(flag.p, seg_id.p, c->cam_obs.p, c->obs_intr.p, c->cam_start.p, no, c->nc,
+                                                                                               c->seg_start.p, c->seg_intr.p, c->cam_seg.p); LAUNCH_CHECK();
+    OMVG_CUDA(cudaStreamSynchronize(s));                      // the temporaries above are released at the end of this scope
+    c->launches += 11;
     tm.lap("device sort / lists");
   }
   if (P->point_fixed) {
@@ -549,7 +575,8 @@ int omvg_ba_create(omvg_ba_ctx **out, int device, const omvg_ba_problem *P) {
   AL(c->sc_pt, 3 * (size_t)c->np); AL(c->sc_cam, 6 * c->nc); AL(c->sc_intr, c->ni8);
   AL(c->diag_pt, 3 * (size_t)c->np); AL(c->diag_cam, 6 * c->nc); AL(c->diag_intr, c->ni8);
   AL(c->lmD_pt, 3 * (size_t)c->np); AL(c->lmD_cam, 6 * c->nc); AL(c->lmD_intr, c->ni8); AL(c->g_cam, 6 * c->nc); AL(c->g_intr, c->ni8);
-  AL(c->EtFi, 3 * KI * (size_t)c->np); AL(c->FtF, 36 * (size_t)c->nc); AL(c->FiFi, 64 * (size_t)c->ni);
+  AL(c->EtFi, 3 * KI * (size_t)c->np); AL(c->FtF, 36 * (size_t)c->nc); AL(c->FiFi, 64 * (size_t)c->ni); AL(c->FiFc, (size_t)c->nseg * KI * 6);
+  AL(c->Gv, (size_t)gv_rec(c->kiu) * c->np);
   AL(c->EtE, 6 * (size_t)c->np); AL(c->Etb, 3 * (size_t)c->np); AL(c->Einv, 9 * (size_t)c->np); AL(c->step_pt, 3 * (size_t)c->np); AL(c->step_red, c->nred);
   AL(c->intr_mask, c->ni);
   AL(c->Sci, (size_t)c->ni8 * 6 * c->nc); AL(c->Sii, (size_t)c->ni8 * c->ni8); AL(c->rhs, c->nred); AL(c->Minv_c, 36 * (size_t)c->nc); AL(c->Minv_i, (size_t)c->ni * KI * KI);
@@ -561,8 +588,15 @@ int omvg_ba_create(omvg_ba_ctx **out, int device, const omvg_ba_problem *P) {
   if (c->npri) { AL(c->rP, 3 * c->npri); AL(c->JP, 18 * c->npri); }
   AL(c->part, std::max(c->eval_blocks, 1024) + 2); AL(c->part2, 1024); AL(c->part3, 1024); c->ics_chunks = (int)std::max<long long>(1, std::min<long long>(4ll * c->n_sms / std::max(1, c->ni), (c->no + 2047) / 2048));
   AL(c->icol_part, (size_t)c->ni * c->ics_chunks * ICS_W); AL(c->scal, S_COUNT); AL(c->fail, 1);
+  c->corner_chunks = (int)std::max<long long>(1, std::min<long long>(4ll * c->n_sms / std::max(1, c->ni), (c->np + CORNER_THREADS - 1) / CORNER_THREADS));
+  AL(c->corner_part, (size_t)c->ni * c->corner_chunks * ICS_W);
 #undef AL
   OMVG_CUDA(cudaMemsetAsync(c->scal.p, 0, S_COUNT * sizeof(double), s));
+  // the border and corner kernels store their blocks on every LM step; the rest of Sci / Sii (groups a pose is not seen
+  // through, unused intrinsic rows, blocks between groups) only the per-observation Schur kernel adds to (n_slow > 0):
+  // zeroed here, and before every step when that kernel runs
+  OMVG_CUDA(cudaMemsetAsync(c->Sci.p, 0, c->Sci.n * sizeof(double), s));
+  OMVG_CUDA(cudaMemsetAsync(c->Sii.p, 0, c->Sii.n * sizeof(double), s));
   tm.lap("allocations");
   if ((rc = build_structure(c))) return rc;
   tm.lap("structure");
@@ -675,39 +709,48 @@ int omvg_ba_run(omvg_ba_ctx *c, const omvg_ba_options *O, omvg_ba_summary *sum) 
     { Diag3 DG{}; DG.s[0] = Diag3Seg{c->diag_pt.p, c->lmD_pt.p, 3 * c->np}; DG.s[1] = Diag3Seg{c->diag_cam.p, c->lmD_cam.p, 6 * c->nc}; DG.s[2] = Diag3Seg{c->diag_intr.p, c->lmD_intr.p, c->ni8};
       const int nb = std::max(1, std::min(2 * c->n_sms, (3 * c->np + 255) / 256));
       lm_diag3_kernel<<<dim3(nb, 3), 256, 0, c->stream>>>(DG, O->min_lm_diagonal, O->max_lm_diagonal, radius); LAUNCH_CHECK(); }
-    // ---- reduced camera system: with free structure schur_stage / schur_gather take the landmarks of the co-visibility
-    // lists and schur_kernel the rest (n_slow); with constant structure schur_kernel adds the border alone
-    if (m.pts_free && !c->corner_rep.p) { if ((rc = c->corner_rep.alloc((size_t)CORNER_REPS * (KI * KI + KI)))) return rc; }
-    // (with free structure schur_gather_kernel writes every block of Scc; rhs is fully written by s_init_kernel)
-    { Zero4 Z{}; Z.p[0] = c->Scc.p; Z.n[0] = m.pts_free ? 0 : (long long)c->nnzb * 36; Z.p[1] = c->Sci.p; Z.n[1] = (long long)c->Sci.n; Z.p[2] = c->Sii.p; Z.n[2] = (long long)c->Sii.n;
-      Z.p[3] = m.pts_free ? c->corner_rep.p : c->rhs.p; Z.n[3] = m.pts_free ? (long long)c->corner_rep.n : 0;
-      const int nb = (int)std::max<long long>(1, std::min<long long>(4 * c->n_sms, (std::max(Z.n[0], Z.n[1]) + 255) / 256));
-      zero4_kernel<<<dim3(nb, 4), 256, 0, c->stream>>>(Z); LAUNCH_CHECK(); }
-    SchurArgs SA{}; SA.r = c->r.p; SA.Jp = c->Jp.p; SA.Jc = c->Jc.p; SA.Ji = c->Ji.p; SA.EtE = c->EtE.p; SA.Etb = c->Etb.p; SA.EtFi = c->EtFi.p; SA.lmD_pt = c->lmD_pt.p; SA.pt_single = c->pt_single.p; SA.FtF = c->FtF.p; SA.FiFi = c->FiFi.p; SA.g_cam = c->g_cam.p; SA.g_intr = c->g_intr.p;
+    // ---- reduced camera system.  schur_stage writes H and the landmarks' {v, G}; schur_gather stores the camera blocks,
+    // schur_border the intrinsics border and the camera right-hand side, corner / corner_final the intrinsics corner and its
+    // right-hand side, all without atomics; then schur_kernel adds the landmarks outside the co-visibility lists (n_slow)
+    // with atomics.  With constant structure the reduced system is its radius-independent part: Scc = diag(Fc'Fc) (stored
+    // by schur_border), Sci = Fi'Fc, Sii = Fi'Fi.
+    { Zero4 Z{}; Z.p[0] = c->Scc.p; Z.n[0] = m.pts_free ? 0 : (long long)c->nnzb * 36;
+      Z.p[1] = c->Sci.p; Z.n[1] = c->n_slow > 0 ? (long long)c->Sci.n : 0; Z.p[2] = c->Sii.p; Z.n[2] = c->n_slow > 0 ? (long long)c->Sii.n : 0;
+      if (Z.n[0] || Z.n[1]) {
+        const int nb = (int)std::max<long long>(1, std::min<long long>(4 * c->n_sms, (std::max(Z.n[0], Z.n[1]) + 255) / 256));
+        zero4_kernel<<<dim3(nb, 3), 256, 0, c->stream>>>(Z); LAUNCH_CHECK(); c->launches++;
+      } }
+    SchurArgs SA{}; SA.Jp = c->Jp.p; SA.Jc = c->Jc.p; SA.Ji = c->Ji.p; SA.EtE = c->EtE.p; SA.Etb = c->Etb.p; SA.EtFi = c->EtFi.p; SA.lmD_pt = c->lmD_pt.p; SA.pt_single = c->pt_single.p;
     SA.obs_pose = c->obs_pose.p; SA.obs_intr = c->obs_intr.p; SA.obs_pt = c->obs_pt.p; SA.pt_start = c->pt_start.p; SA.n = c->no; SA.n_poses = c->nc; SA.n_intr = c->ni;
-    SA.pts_free = m.pts_free; SA.kiu = c->kiu; SA.bsr = Bsr{c->bitmap.p, c->wprefix.p, c->rowptr.p, c->words}; SA.Scc = c->Scc.p; SA.Sci = c->Sci.p; SA.Sii = c->Sii.p; SA.rhs = c->rhs.p;
+    SA.kiu = c->kiu; SA.bsr = Bsr{c->bitmap.p, c->wprefix.p, c->rowptr.p, c->words}; SA.Scc = c->Scc.p; SA.Sci = c->Sci.p; SA.Sii = c->Sii.p; SA.rhs = c->rhs.p;
     SA.Einv = c->Einv.p; SA.fail = c->fail.p;
-    { SchurArgs SI = SA; if (m.pts_free) SI.Scc = nullptr;
-      const int ninit = std::max(std::max(36 * c->nc, 64 * c->ni), c->nred); s_init_kernel<<<(ninit + 255) / 256, 256, 0, c->stream>>>(SI); LAUNCH_CHECK(); }
+    const BorderArgs BA{m.pts_free ? c->H.p : nullptr, c->Gv.p, c->FiFc.p, c->g_cam.p, c->FtF.p, c->cam_seg.p, c->seg_start.p, c->seg_intr.p, c->cam_obs.p, c->obs_pt.p,
+                        c->nc, c->Sci.p, c->rhs.p, m.pts_free ? nullptr : c->Scc.p, SA.bsr};
+    const unsigned sg = (unsigned)((c->no + SCHUR_THREADS - 1) / SCHUR_THREADS);
+    const dim3 cg(c->corner_chunks, c->ni);
+    // (kernels instantiated for the intrinsic columns in use, as the column sums are)
+#define STAGE(K) schur_stage_kernel<K><<<sg, SCHUR_THREADS, 0, c->stream>>>(SA, c->H.p, c->Gv.p)
+#define BORDER(K) schur_border_kernel<K><<<c->nc, CCS_THREADS, 0, c->stream>>>(BA)
+#define CORNER(K) corner_kernel<K><<<cg, CORNER_THREADS, 0, c->stream>>>(c->Gv.p, c->pt_start.p, c->pt_single.p, c->obs_intr.p, c->np, c->corner_chunks, c->corner_part.p)
+#define KIU_SWITCH(L) switch (c->kiu) { case 3: L(3); break; case 4: L(4); break; case 6: L(6); break; case 7: L(7); break; default: L(8); break; }
     if (m.pts_free) {
-      const unsigned sg = (unsigned)((c->no + SCHUR_THREADS - 1) / SCHUR_THREADS);
-      switch (c->kiu) {        // intrinsic columns in use (as for the column sums)
-        case 3: schur_stage_kernel<3><<<sg, SCHUR_THREADS, 0, c->stream>>>(SA, c->H.p, c->corner_rep.p); break;
-        case 4: schur_stage_kernel<4><<<sg, SCHUR_THREADS, 0, c->stream>>>(SA, c->H.p, c->corner_rep.p); break;
-        case 6: schur_stage_kernel<6><<<sg, SCHUR_THREADS, 0, c->stream>>>(SA, c->H.p, c->corner_rep.p); break;
-        case 7: schur_stage_kernel<7><<<sg, SCHUR_THREADS, 0, c->stream>>>(SA, c->H.p, c->corner_rep.p); break;
-        default: schur_stage_kernel<8><<<sg, SCHUR_THREADS, 0, c->stream>>>(SA, c->H.p, c->corner_rep.p); break;
-      }
-      LAUNCH_CHECK();
-      corner_fold_kernel<<<1, 96, 0, c->stream>>>(c->corner_rep.p, c->obs_intr.p, c->nc, c->ni, c->Sii.p, c->rhs.p); LAUNCH_CHECK(); c->launches++;
+      KIU_SWITCH(STAGE); LAUNCH_CHECK();
       GatherArgs G{c->H.p, c->FtF.p, c->pair.p, c->pair_start.p, c->chunk_blk.p, c->chunk_first.p, c->brow.p, c->cols.p, SA.bsr, c->Scc.p, c->gpart.p, c->ticket.p, c->n_chunks};
-      schur_gather_kernel<<<(c->n_chunks + 7) / 8, 256, 0, c->stream>>>(G); LAUNCH_CHECK(); c->launches += 2;
+      schur_gather_kernel<<<(c->n_chunks + 7) / 8, 256, 0, c->stream>>>(G); LAUNCH_CHECK();
+      KIU_SWITCH(CORNER); LAUNCH_CHECK();
+      c->launches += 3;
     }
-    if (!m.pts_free || c->n_slow > 0) {
-      schur_kernel<<<(unsigned)((c->no + SCHUR_THREADS - 1) / SCHUR_THREADS), SCHUR_THREADS, 0, c->stream>>>(SA); LAUNCH_CHECK();
-      mirror_kernel<<<(c->nc * 32 + 255) / 256, 256, 0, c->stream>>>(c->Scc.p, SA.bsr, c->cols.p, c->nc); LAUNCH_CHECK(); c->launches++;
+    KIU_SWITCH(BORDER); LAUNCH_CHECK();
+    corner_final_kernel<<<c->ni * 72, 128, 0, c->stream>>>(m.pts_free ? c->corner_part.p : nullptr, c->corner_chunks, c->nc, c->ni, c->FiFi.p, c->g_intr.p, c->Sii.p, c->rhs.p); LAUNCH_CHECK();
+    c->launches += 2;
+#undef STAGE
+#undef BORDER
+#undef CORNER
+#undef KIU_SWITCH
+    if (m.pts_free && c->n_slow > 0) {
+      schur_kernel<<<sg, SCHUR_THREADS, 0, c->stream>>>(SA); LAUNCH_CHECK();
+      mirror_kernel<<<(c->nc * 32 + 255) / 256, 256, 0, c->stream>>>(c->Scc.p, SA.bsr, c->cols.p, c->nc); LAUNCH_CHECK(); c->launches += 2;
     }
-    c->launches++;
     finish_cam_kernel<<<(c->nc + 63) / 64, 64, 0, c->stream>>>(c->Scc.p, SA.bsr, c->lmD_cam.p, m.pose_mask, c->nc, c->Minv_c.p, c->fail.p, use_dense ? 0 : 1); LAUNCH_CHECK();
     finish_intr_kernel<<<1, 256, 0, c->stream>>>(c->Sii.p, c->lmD_intr.p, c->intr_mask.p, c->ni8, c->Minv_i.p, c->work_i.p, c->fail.p, (use_block_pcg || use_dense) ? 0 : 1); LAUNCH_CHECK();
     // ---- PCG on S z = rhs
@@ -816,7 +859,7 @@ int omvg_ba_run(omvg_ba_ctx *c, const omvg_ba_options *O, omvg_ba_summary *sum) 
     negate_kernel<<<(c->nred + 255) / 256, 256, 0, c->stream>>>(c->z.p, c->nred, c->step_red.p); LAUNCH_CHECK();
     // ---- model cost change
     model_kernel<<<c->eval_blocks, MODEL_THREADS, 0, c->stream>>>(c->r.p, c->Jp.p, c->Jc.p, c->Ji.p, c->obs_pose.p, c->obs_intr.p, c->obs_pt.p, c->no, c->nc, c->kiu, c->step_pt.p, c->step_red.p, c->part.p); LAUNCH_CHECK();
-    c->launches += 8;
+    c->launches += 6;
     if (c->npri) { prior_model_kernel<<<1, PRIOR_THREADS, 0, c->stream>>>(c->JP.p, c->rP.p, c->prior_pose.p, c->npri, c->step_red.p, c->part.p + c->eval_blocks); LAUNCH_CHECK(); c->launches++; }
     if ((rc = reduce_to(c, c->part.p, c->eval_blocks + (c->npri ? 1 : 0), S_MODEL))) return rc;
     // ---- candidate = Plus(x, step * scale)

@@ -11,7 +11,9 @@
 //   point_accum_kernel  SchurEliminator::ChunkDiagonalBlockAndGradient (schur_eliminator_impl.h:434-490)
 //   colsum_kernel       SquaredColumnNorm / gradient for the camera+intrinsic columns
 //   schur_stage_kernel  SchurEliminator::Eliminate (schur_eliminator_impl.h:176-298, :374-410, :499-548):
-//   schur_gather_kernel   per-observation terms, then the camera blocks as sums over co-visibility lists;
+//   schur_gather_kernel   per-observation and per-landmark terms, then the camera blocks, the intrinsics border and
+//   schur_border_kernel   the camera right-hand side, the intrinsics corner as fixed-order sums;
+//   corner_kernel         (+ corner_final_kernel)
 //   schur_kernel          the same elimination with atomics for the landmarks the lists leave out
 //   pcg3_kernel         ConjugateGradientsSolver::Solve (conjugate_gradients_solver.cc:66-245) with a two-level
 //   pcg5_kernel         preconditioner (block-Jacobi + aggregated gauge space), standing in for SimplicialLDLT
@@ -176,6 +178,26 @@ __global__ void setup_single_kernel(const int *__restrict__ s_intr, const int *_
   pt_single[j] = one;
   const int K = pt_start[j + 1] - pt_start[j];
   if (K > 0 && (!one || K > 32)) atomicAdd(n_slow, 1);
+}
+// dst[t] = src[perm[t]]
+__global__ void setup_permute_kernel(const int *__restrict__ perm, const int *__restrict__ src, long long n, int *__restrict__ dst) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < n) dst[t] = src[perm[t]];
+}
+// Segments of the per-pose lists (ordered by pose, then intrinsic group): flag[t] = a new (pose, group) starts at t;
+// flag[n] = 0, so that the exclusive scan of the flags ends with the segment count
+__global__ void setup_seg_flag_kernel(const int *__restrict__ pose_key, const int *__restrict__ cam_obs, const int *__restrict__ obs_intr, long long n, int *__restrict__ flag) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t > n) return;
+  flag[t] = t < n && (t == 0 || pose_key[t] != pose_key[t - 1] || obs_intr[cam_obs[t]] != obs_intr[cam_obs[t - 1]]);
+}
+// seg_start[nseg + 1], seg_intr[nseg] from the flags and their exclusive scan seg_id; cam_seg[p] = first segment of pose p
+__global__ void setup_seg_emit_kernel(const int *__restrict__ flag, const int *__restrict__ seg_id, const int *__restrict__ cam_obs, const int *__restrict__ obs_intr,
+                                      const int *__restrict__ cam_start, long long n, int n_poses, int *__restrict__ seg_start, int *__restrict__ seg_intr, int *__restrict__ cam_seg) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < n && flag[t]) { seg_start[seg_id[t]] = (int)t; seg_intr[seg_id[t]] = obs_intr[cam_obs[t]]; }
+  if (t == n) seg_start[seg_id[n]] = (int)n;
+  if (t <= n_poses) cam_seg[t] = seg_id[cam_start[t]];
 }
 
 // ------------------------------------------------------------------------------ outlier rejection on the resident scene
@@ -523,49 +545,69 @@ __global__ void point_accum_kernel(const double *__restrict__ Jp, const double *
 // pose's observation list — fixed order (lane, then warp), no atomics.  One warp per pose left 7 warps per SM at 1000
 // poses and a 16-deep chain of dependent gathers: 82 us at 1000 cameras, 43 us at 10.
 constexpr int CCS_THREADS = 128;
-__global__ void __launch_bounds__(CCS_THREADS) cam_colsum_kernel(const double *__restrict__ Jc, const double *__restrict__ r, const int *__restrict__ cam_start,
-                                  const int *__restrict__ cam_obs, int n_poses, long long n, double *__restrict__ diag_cam,
-                                  double *__restrict__ g_cam, double *__restrict__ FtF) {
-  __shared__ double sh[CCS_THREADS / 32][27];
-  const int p = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (p >= n_poses) return;
-  double m[21], g[6] = {0, 0, 0, 0, 0, 0};
+// fixed-order sum of v[0..N) over the CCS_THREADS threads of a CTA (shuffle tree per warp, then the warps in order);
+// the N sums are left in sh[0..N) (sh: CCS_THREADS / 32 * N doubles).  Ends with a barrier.
+template <int N> __device__ __forceinline__ void cta_sum(double (&v)[N], double *sh) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   #pragma unroll
-  for (int k = 0; k < 21; ++k) m[k] = 0.0;
-  for (int t = cam_start[p] + threadIdx.x; t < cam_start[p + 1]; t += CCS_THREADS) {
-    const long long o = cam_obs[t];
-    const double r0 = r[o], r1 = r[n + o];
-    double a[6], b[6];
-    #pragma unroll
-    for (int k = 0; k < 6; ++k) { a[k] = Jc[k * n + o]; b[k] = Jc[(6 + k) * n + o]; g[k] += a[k] * r0 + b[k] * r1; }
-    int q = 0;
-    #pragma unroll
-    for (int i = 0; i < 6; ++i)
-      #pragma unroll
-      for (int k = 0; k <= i; ++k) m[q++] += a[i] * a[k] + b[i] * b[k];
-  }
-  #pragma unroll
-  for (int k = 0; k < 21; ++k) { for (int o = 16; o > 0; o >>= 1) m[k] += __shfl_down_sync(0xffffffffu, m[k], o); }
-  #pragma unroll
-  for (int k = 0; k < 6; ++k) { for (int o = 16; o > 0; o >>= 1) g[k] += __shfl_down_sync(0xffffffffu, g[k], o); }
+  for (int k = 0; k < N; ++k) { for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_down_sync(0xffffffffu, v[k], o); }
   if (lane == 0) {
     #pragma unroll
-    for (int k = 0; k < 21; ++k) sh[warp][k] = m[k];
-    #pragma unroll
-    for (int k = 0; k < 6; ++k) sh[warp][21 + k] = g[k];
+    for (int k = 0; k < N; ++k) sh[warp * N + k] = v[k];
   }
   __syncthreads();
-  if (threadIdx.x < 27) {
-    double v = 0.0;
+  if (threadIdx.x < N) {
+    double s = 0.0;
     #pragma unroll
-    for (int w = 0; w < CCS_THREADS / 32; ++w) v += sh[w][threadIdx.x];
-    sh[0][threadIdx.x] = v;
+    for (int w = 0; w < CCS_THREADS / 32; ++w) s += sh[w * N + threadIdx.x];
+    sh[threadIdx.x] = s;
   }
   __syncthreads();
+}
+// The pose's list is ordered by intrinsic group (segments cam_seg[p] .. cam_seg[p+1] of seg_start / seg_intr), and per
+// segment (pose c, group q) the kernel also stores the border term FiFc[seg] = sum Fi'Fc (KIU x 6, row stride 6, KI rows
+// reserved): it does not depend on the LM radius, so schur_border_kernel reads it once per LM step.
+template <int KIU>
+__global__ void __launch_bounds__(CCS_THREADS) cam_colsum_kernel(const double *__restrict__ Jc, const double *__restrict__ Ji, const double *__restrict__ r,
+                                  const int *__restrict__ cam_seg, const int *__restrict__ seg_start, const int *__restrict__ cam_obs, int n_poses, long long n,
+                                  double *__restrict__ diag_cam, double *__restrict__ g_cam, double *__restrict__ FtF, double *__restrict__ FiFc) {
+  __shared__ double sh[CCS_THREADS / 32 * (KIU * 6 > 27 ? KIU * 6 : 27)];
+  const int p = blockIdx.x;
+  if (p >= n_poses) return;
+  double m[27];                                        // Fc'Fc lower triangle (21), then Fc'r (6)
+  #pragma unroll
+  for (int k = 0; k < 27; ++k) m[k] = 0.0;
+  for (int s = cam_seg[p]; s < cam_seg[p + 1]; ++s) {
+    double f[KIU * 6];
+    #pragma unroll
+    for (int k = 0; k < KIU * 6; ++k) f[k] = 0.0;
+    for (int t = seg_start[s] + threadIdx.x; t < seg_start[s + 1]; t += CCS_THREADS) {
+      const long long o = cam_obs[t];
+      const double r0 = r[o], r1 = r[n + o];
+      double a[6], b[6];
+      #pragma unroll
+      for (int k = 0; k < 6; ++k) { a[k] = Jc[k * n + o]; b[k] = Jc[(6 + k) * n + o]; m[21 + k] += a[k] * r0 + b[k] * r1; }
+      int q = 0;
+      #pragma unroll
+      for (int i = 0; i < 6; ++i)
+        #pragma unroll
+        for (int k = 0; k <= i; ++k) m[q++] += a[i] * a[k] + b[i] * b[k];
+      #pragma unroll
+      for (int i = 0; i < KIU; ++i) {
+        const double u0 = Ji[i * n + o], u1 = Ji[(KI + i) * n + o];
+        #pragma unroll
+        for (int k = 0; k < 6; ++k) f[6 * i + k] += u0 * a[k] + u1 * b[k];
+      }
+    }
+    cta_sum<KIU * 6>(f, sh);
+    if (threadIdx.x < KIU * 6) FiFc[(size_t)s * KI * 6 + threadIdx.x] = sh[threadIdx.x];
+    __syncthreads();
+  }
+  cta_sum<27>(m, sh);
   if (threadIdx.x == 0) {
     int q = 0;
-    for (int i = 0; i < 6; ++i) for (int k = 0; k <= i; ++k) { FtF[36 * (size_t)p + i * 6 + k] = sh[0][q]; FtF[36 * (size_t)p + k * 6 + i] = sh[0][q]; ++q; }
-    for (int k = 0; k < 6; ++k) { diag_cam[6 * p + k] = FtF[36 * (size_t)p + k * 6 + k]; g_cam[6 * p + k] = sh[0][21 + k]; }
+    for (int i = 0; i < 6; ++i) for (int k = 0; k <= i; ++k) { FtF[36 * (size_t)p + i * 6 + k] = sh[q]; FtF[36 * (size_t)p + k * 6 + i] = sh[q]; ++q; }
+    for (int k = 0; k < 6; ++k) { diag_cam[6 * p + k] = FtF[36 * (size_t)p + k * 6 + k]; g_cam[6 * p + k] = sh[21 + k]; }
   }
 }
 
@@ -672,10 +714,9 @@ __global__ void bitmap_cols_kernel(const unsigned *__restrict__ bitmap, const in
 }
 
 struct SchurArgs {
-  const double *r, *Jp, *Jc, *Ji, *EtE, *Etb, *EtFi, *lmD_pt;
+  const double *Jp, *Jc, *Ji, *EtE, *Etb, *EtFi, *lmD_pt;
   const int *obs_pose, *obs_intr, *obs_pt, *pt_start; const unsigned char *pt_single;
-  const double *FtF, *FiFi, *g_cam, *g_intr;
-  long long n; int n_poses, n_intr, pts_free, kiu;
+  long long n; int n_poses, n_intr, kiu;
   Bsr bsr;
   double *Scc;      // [nnzb][36]
   double *Sci;      // [KI*n_intr][6*n_poses]
@@ -685,23 +726,11 @@ struct SchurArgs {
   int *fail;
 };
 
-// Radius-independent part of the reduced system, computed once per Jacobian evaluation without atomics
-// (cam_colsum / intr_colsum): Scc(p,p) = Fc'Fc, Sii(q,q) = Fi'Fi, rhs = [Fc'r ; Fi'r].  S must be zeroed first.
-// With A.Scc null the camera blocks are left alone (schur_gather_kernel writes Scc(p,p) = Fc'Fc - sum itself).
-__global__ void s_init_kernel(SchurArgs A) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int nc36 = 36 * A.n_poses, ni64 = 64 * A.n_intr, nred = 6 * A.n_poses + KI * A.n_intr;
-  if (i < nc36 && A.Scc) { const int p = i / 36; A.Scc[36 * (size_t)bsr_find(A.bsr, p, p) + i % 36] = A.FtF[i]; }
-  if (i < ni64) { const int q = i / 64, e = i % 64; A.Sii[(size_t)(KI * q + e / KI) * (KI * A.n_intr) + KI * q + e % KI] = A.FiFi[i]; }
-  if (i < nred) A.rhs[i] = i < 6 * A.n_poses ? A.g_cam[i] : A.g_intr[i - 6 * A.n_poses];
-}
-
-// One thread per observation t.  Adds the point-elimination terms  -(E'F)' (E'E + D^2)^-1 (E'F)  and the
-// same-observation border term Fi'Fc.  Camera-pair blocks are accumulated for cam(u) >= cam(t) only
-// (mirror_kernel fills the lower triangle); everything hot (the intrinsics corner, its right-hand side) is
-// reduced per point first so that no address sees more than ~one atomic per point.
-// With free structure it takes only the landmarks schur_stage / schur_gather leave (several intrinsic groups or more
-// than 32 views); with constant structure it adds the border Fi'Fc of every observation.
+// One thread per observation t of the landmarks schur_stage / schur_gather leave (several intrinsic groups or more than
+// 32 views).  Adds their point-elimination terms  -(E'F)' (E'E + D^2)^-1 (E'F)  to what schur_gather, schur_border and
+// corner_final have stored.  Camera-pair blocks are accumulated for cam(u) >= cam(t) only (mirror_kernel fills the
+// lower triangle); the intrinsics corner and its right-hand side are reduced per point first so that no address sees
+// more than ~one atomic per point.
 constexpr int SCHUR_THREADS = 128;
 __global__ void __launch_bounds__(SCHUR_THREADS) schur_kernel(SchurArgs A) {
   __shared__ double s_ii[KI * KI + KI];
@@ -714,7 +743,7 @@ __global__ void __launch_bounds__(SCHUR_THREADS) schur_kernel(SchurArgs A) {
   const int q0 = s_q0;
   const int nred_c = 6 * A.n_poses, ni8 = KI * A.n_intr;
   bool mine = t < n;
-  if (mine && A.pts_free) { const int j = A.obs_pt[t]; mine = !(A.pt_single[j] != 0 && A.pt_start[j + 1] - A.pt_start[j] <= 32); }
+  if (mine) { const int j = A.obs_pt[t]; mine = !(A.pt_single[j] != 0 && A.pt_start[j + 1] - A.pt_start[j] <= 32); }
   if (mine) {
     const int j = A.obs_pt[t], ct = A.obs_pose[t], qt = A.obs_intr[t];
     double jc[12], ji[2 * KI], jp[6];
@@ -725,108 +754,96 @@ __global__ void __launch_bounds__(SCHUR_THREADS) schur_kernel(SchurArgs A) {
     #pragma unroll
     for (int k = 0; k < 6; ++k) jp[k] = A.Jp[k * n + t];
     double *sci_row0 = A.Sci + (size_t)(KI * qt) * nred_c + 6 * ct;
-    if (!A.pts_free) {
+    double inv[9], ie[3], m[6];
+    const double *E = A.EtE + 6 * (size_t)j;
+    const double d0 = A.lmD_pt[3 * j], d1 = A.lmD_pt[3 * j + 1], d2 = A.lmD_pt[3 * j + 2];
+    m[0] = E[0] + d0 * d0; m[1] = E[1]; m[2] = E[2] + d1 * d1; m[3] = E[3]; m[4] = E[4]; m[5] = E[5] + d2 * d2;
+    const bool ok = inv3_spd(m, inv);
+    if (!ok) atomicExch(A.fail, 1);
+    const double *eb = A.Etb + 3 * (size_t)j;
+    #pragma unroll
+    for (int a = 0; a < 3; ++a) ie[a] = inv[a * 3] * eb[0] + inv[a * 3 + 1] * eb[1] + inv[a * 3 + 2] * eb[2];
+    const bool first = t == A.pt_start[j];
+    if (first) { for (int a = 0; a < 9; ++a) A.Einv[9 * (size_t)j + a] = inv[a]; }
+    double efc[18];                                          // E'Fc of this observation (3x6)
+    #pragma unroll
+    for (int a = 0; a < 3; ++a)
+      #pragma unroll
+      for (int c = 0; c < 6; ++c) efc[a * 6 + c] = jp[a] * jc[c] + jp[3 + a] * jc[6 + c];
+    // rhs_c -= (E'Fc)' (Einv E'b)
+    #pragma unroll
+    for (int c = 0; c < 6; ++c) atomicAdd(&A.rhs[6 * ct + c], -(efc[c] * ie[0] + efc[6 + c] * ie[1] + efc[12 + c] * ie[2]));
+    const bool single = A.pt_single[j] != 0;
+    if (single) {
+      // border with the point-summed E'Fi:  Sci(qt; ct) -= (Einv E'Fi_pt)' E'Fc
+      const double *fi = A.EtFi + (size_t)j * 3 * KI;
       #pragma unroll
       for (int a = 0; a < KI; ++a) {
-        if (ji[a] == 0.0 && ji[KI + a] == 0.0) continue;
+        const double f0 = fi[a], f1 = fi[KI + a], f2 = fi[2 * KI + a];
+        if (f0 == 0.0 && f1 == 0.0 && f2 == 0.0) continue;   // constant parameter
+        const double g0 = inv[0] * f0 + inv[1] * f1 + inv[2] * f2, g1 = inv[3] * f0 + inv[4] * f1 + inv[5] * f2, g2 = inv[6] * f0 + inv[7] * f1 + inv[8] * f2;
         #pragma unroll
-        for (int b = 0; b < 6; ++b) atomicAdd(&sci_row0[(size_t)a * nred_c + b], ji[a] * jc[b] + ji[KI + a] * jc[6 + b]);
-      }
-    } else {
-      double inv[9], ie[3], m[6];
-      const double *E = A.EtE + 6 * (size_t)j;
-      const double d0 = A.lmD_pt[3 * j], d1 = A.lmD_pt[3 * j + 1], d2 = A.lmD_pt[3 * j + 2];
-      m[0] = E[0] + d0 * d0; m[1] = E[1]; m[2] = E[2] + d1 * d1; m[3] = E[3]; m[4] = E[4]; m[5] = E[5] + d2 * d2;
-      const bool ok = inv3_spd(m, inv);
-      if (!ok) atomicExch(A.fail, 1);
-      const double *eb = A.Etb + 3 * (size_t)j;
-      #pragma unroll
-      for (int a = 0; a < 3; ++a) ie[a] = inv[a * 3] * eb[0] + inv[a * 3 + 1] * eb[1] + inv[a * 3 + 2] * eb[2];
-      const bool first = t == A.pt_start[j];
-      if (first) { for (int a = 0; a < 9; ++a) A.Einv[9 * (size_t)j + a] = inv[a]; }
-      double efc[18];                                          // E'Fc of this observation (3x6)
-      #pragma unroll
-      for (int a = 0; a < 3; ++a)
-        #pragma unroll
-        for (int c = 0; c < 6; ++c) efc[a * 6 + c] = jp[a] * jc[c] + jp[3 + a] * jc[6 + c];
-      // rhs_c -= (E'Fc)' (Einv E'b)
-      #pragma unroll
-      for (int c = 0; c < 6; ++c) atomicAdd(&A.rhs[6 * ct + c], -(efc[c] * ie[0] + efc[6 + c] * ie[1] + efc[12 + c] * ie[2]));
-      const bool single = A.pt_single[j] != 0;
-      if (single) {
-        // border with the point-summed E'Fi:  Sci(qt; ct) += Fi'Fc - (Einv E'Fi_pt)' E'Fc
-        const double *fi = A.EtFi + (size_t)j * 3 * KI;
-        #pragma unroll
-        for (int a = 0; a < KI; ++a) {
-          const double f0 = fi[a], f1 = fi[KI + a], f2 = fi[2 * KI + a];
-          if (f0 == 0.0 && f1 == 0.0 && f2 == 0.0 && ji[a] == 0.0 && ji[KI + a] == 0.0) continue;   // constant parameter
-          const double g0 = inv[0] * f0 + inv[1] * f1 + inv[2] * f2, g1 = inv[3] * f0 + inv[4] * f1 + inv[5] * f2, g2 = inv[6] * f0 + inv[7] * f1 + inv[8] * f2;
+        for (int b = 0; b < 6; ++b)
+          atomicAdd(&sci_row0[(size_t)a * nred_c + b], -(g0 * efc[b] + g1 * efc[6 + b] + g2 * efc[12 + b]));
+        if (first) {                                          // once per point: corner and its right-hand side
+          const double rv = -(f0 * ie[0] + f1 * ie[1] + f2 * ie[2]);
+          if (qt == q0) atomicAdd(&s_ii[KI * KI + a], rv); else atomicAdd(&A.rhs[nred_c + KI * qt + a], rv);
           #pragma unroll
-          for (int b = 0; b < 6; ++b)
-            atomicAdd(&sci_row0[(size_t)a * nred_c + b], ji[a] * jc[b] + ji[KI + a] * jc[6 + b] - (g0 * efc[b] + g1 * efc[6 + b] + g2 * efc[12 + b]));
-          if (first) {                                          // once per point: corner and its right-hand side
-            const double rv = -(f0 * ie[0] + f1 * ie[1] + f2 * ie[2]);
-            if (qt == q0) atomicAdd(&s_ii[KI * KI + a], rv); else atomicAdd(&A.rhs[nred_c + KI * qt + a], rv);
-            #pragma unroll
-            for (int b = 0; b < KI; ++b) {
-              const double v = -(g0 * fi[b] + g1 * fi[KI + b] + g2 * fi[2 * KI + b]);
-              if (v == 0.0) continue;
-              if (qt == q0) atomicAdd(&s_ii[a * KI + b], v); else atomicAdd(&A.Sii[(size_t)(KI * qt + a) * ni8 + KI * qt + b], v);
-            }
+          for (int b = 0; b < KI; ++b) {
+            const double v = -(g0 * fi[b] + g1 * fi[KI + b] + g2 * fi[2 * KI + b]);
+            if (v == 0.0) continue;
+            if (qt == q0) atomicAdd(&s_ii[a * KI + b], v); else atomicAdd(&A.Sii[(size_t)(KI * qt + a) * ni8 + KI * qt + b], v);
           }
         }
       }
-      double gt_c[18];                                         // Einv * E'Fc_t
+    }
+    double gt_c[18];                                         // Einv * E'Fc_t
+    #pragma unroll
+    for (int a = 0; a < 3; ++a)
+      #pragma unroll
+      for (int c = 0; c < 6; ++c) gt_c[a * 6 + c] = inv[a * 3] * efc[c] + inv[a * 3 + 1] * efc[6 + c] + inv[a * 3 + 2] * efc[12 + c];
+    double gt_i[3 * KI];
+    if (!single) {                                           // general (rare) path: per-observation-pair border terms
+      #pragma unroll
+      for (int a = 0; a < KI; ++a) {
+        const double e0 = jp[0] * ji[a] + jp[3] * ji[KI + a], e1 = jp[1] * ji[a] + jp[4] * ji[KI + a], e2 = jp[2] * ji[a] + jp[5] * ji[KI + a];
+        gt_i[a] = inv[0] * e0 + inv[1] * e1 + inv[2] * e2; gt_i[KI + a] = inv[3] * e0 + inv[4] * e1 + inv[5] * e2; gt_i[2 * KI + a] = inv[6] * e0 + inv[7] * e1 + inv[8] * e2;
+        const double rv = -(e0 * ie[0] + e1 * ie[1] + e2 * ie[2]);
+        if (rv != 0.0) atomicAdd(&A.rhs[nred_c + KI * qt + a], rv);
+      }
+    }
+    for (long long u = A.pt_start[j]; u < A.pt_start[j + 1]; ++u) {
+      const int cu = A.obs_pose[u];
+      if (cu < ct && single) continue;
+      double up[6], uc[12], efu[18];
+      #pragma unroll
+      for (int k = 0; k < 6; ++k) up[k] = A.Jp[k * n + u];
+      #pragma unroll
+      for (int k = 0; k < 12; ++k) uc[k] = A.Jc[k * n + u];
       #pragma unroll
       for (int a = 0; a < 3; ++a)
         #pragma unroll
-        for (int c = 0; c < 6; ++c) gt_c[a * 6 + c] = inv[a * 3] * efc[c] + inv[a * 3 + 1] * efc[6 + c] + inv[a * 3 + 2] * efc[12 + c];
-      double gt_i[3 * KI];
-      if (!single) {                                           // general (rare) path: per-observation-pair border terms
+        for (int c = 0; c < 6; ++c) efu[a * 6 + c] = up[a] * uc[c] + up[3 + a] * uc[6 + c];
+      if (cu >= ct) {                                        // Scc(ct, cu) -= (Einv E'Fc_t)' E'Fc_u
+        double *blk = A.Scc + 36 * (size_t)bsr_find(A.bsr, ct, cu);
+        #pragma unroll
+        for (int a = 0; a < 6; ++a)
+          #pragma unroll
+          for (int b = 0; b < 6; ++b) atomicAdd(&blk[a * 6 + b], -(gt_c[a] * efu[b] + gt_c[6 + a] * efu[6 + b] + gt_c[12 + a] * efu[12 + b]));
+      }
+      if (!single) {
+        const int qu = A.obs_intr[u];
         #pragma unroll
         for (int a = 0; a < KI; ++a) {
-          const double e0 = jp[0] * ji[a] + jp[3] * ji[KI + a], e1 = jp[1] * ji[a] + jp[4] * ji[KI + a], e2 = jp[2] * ji[a] + jp[5] * ji[KI + a];
-          gt_i[a] = inv[0] * e0 + inv[1] * e1 + inv[2] * e2; gt_i[KI + a] = inv[3] * e0 + inv[4] * e1 + inv[5] * e2; gt_i[2 * KI + a] = inv[6] * e0 + inv[7] * e1 + inv[8] * e2;
-          const double rv = -(e0 * ie[0] + e1 * ie[1] + e2 * ie[2]);
-          if (rv != 0.0) atomicAdd(&A.rhs[nred_c + KI * qt + a], rv);
-          if (ji[a] == 0.0 && ji[KI + a] == 0.0) continue;
+          if (gt_i[a] == 0.0 && gt_i[KI + a] == 0.0 && gt_i[2 * KI + a] == 0.0) continue;
           #pragma unroll
-          for (int b = 0; b < 6; ++b) atomicAdd(&sci_row0[(size_t)a * nred_c + b], ji[a] * jc[b] + ji[KI + a] * jc[6 + b]);
-        }
-      }
-      for (long long u = A.pt_start[j]; u < A.pt_start[j + 1]; ++u) {
-        const int cu = A.obs_pose[u];
-        if (cu < ct && single) continue;
-        double up[6], uc[12], efu[18];
-        #pragma unroll
-        for (int k = 0; k < 6; ++k) up[k] = A.Jp[k * n + u];
-        #pragma unroll
-        for (int k = 0; k < 12; ++k) uc[k] = A.Jc[k * n + u];
-        #pragma unroll
-        for (int a = 0; a < 3; ++a)
+          for (int b = 0; b < 6; ++b) atomicAdd(&A.Sci[(size_t)(KI * qt + a) * nred_c + 6 * cu + b], -(gt_i[a] * efu[b] + gt_i[KI + a] * efu[6 + b] + gt_i[2 * KI + a] * efu[12 + b]));
           #pragma unroll
-          for (int c = 0; c < 6; ++c) efu[a * 6 + c] = up[a] * uc[c] + up[3 + a] * uc[6 + c];
-        if (cu >= ct) {                                        // Scc(ct, cu) -= (Einv E'Fc_t)' E'Fc_u
-          double *blk = A.Scc + 36 * (size_t)bsr_find(A.bsr, ct, cu);
-          #pragma unroll
-          for (int a = 0; a < 6; ++a)
-            #pragma unroll
-            for (int b = 0; b < 6; ++b) atomicAdd(&blk[a * 6 + b], -(gt_c[a] * efu[b] + gt_c[6 + a] * efu[6 + b] + gt_c[12 + a] * efu[12 + b]));
-        }
-        if (!single) {
-          const int qu = A.obs_intr[u];
-          #pragma unroll
-          for (int a = 0; a < KI; ++a) {
-            if (gt_i[a] == 0.0 && gt_i[KI + a] == 0.0 && gt_i[2 * KI + a] == 0.0) continue;
-            #pragma unroll
-            for (int b = 0; b < 6; ++b) atomicAdd(&A.Sci[(size_t)(KI * qt + a) * nred_c + 6 * cu + b], -(gt_i[a] * efu[b] + gt_i[KI + a] * efu[6 + b] + gt_i[2 * KI + a] * efu[12 + b]));
-            #pragma unroll
-            for (int b = 0; b < KI; ++b) {
-              const double ui0 = b < A.kiu ? A.Ji[b * n + u] : 0.0, ui1 = b < A.kiu ? A.Ji[(KI + b) * n + u] : 0.0;
-              const double e0 = up[0] * ui0 + up[3] * ui1, e1 = up[1] * ui0 + up[4] * ui1, e2 = up[2] * ui0 + up[5] * ui1;
-              const double v = gt_i[a] * e0 + gt_i[KI + a] * e1 + gt_i[2 * KI + a] * e2;
-              if (v != 0.0) atomicAdd(&A.Sii[(size_t)(KI * qt + a) * ni8 + KI * qu + b], -v);
-            }
+          for (int b = 0; b < KI; ++b) {
+            const double ui0 = b < A.kiu ? A.Ji[b * n + u] : 0.0, ui1 = b < A.kiu ? A.Ji[(KI + b) * n + u] : 0.0;
+            const double e0 = up[0] * ui0 + up[3] * ui1, e1 = up[1] * ui0 + up[4] * ui1, e2 = up[2] * ui0 + up[5] * ui1;
+            const double v = gt_i[a] * e0 + gt_i[KI + a] * e1 + gt_i[2 * KI + a] * e2;
+            if (v != 0.0) atomicAdd(&A.Sii[(size_t)(KI * qt + a) * ni8 + KI * qu + b], -v);
           }
         }
       }
@@ -843,100 +860,85 @@ __global__ void __launch_bounds__(SCHUR_THREADS) schur_kernel(SchurArgs A) {
 }
 
 // ---- Schur step of the landmarks seen through one intrinsic group by at most 32 views (all other landmarks take
-// schur_kernel).  With E'E + D^2 = L L' per landmark and
-// H_t = L^-1 E'Fc_t (3 x 6) per observation, a camera block is a plain sum  Scc(a,b) = [a == b] Fc'Fc - sum H_t' H_u
-// over the observation pairs (t, u) of one landmark with cam(t) = a, cam(u) = b.  The pairs of every block are listed
-// once per problem (pair_count / pair_emit, sorted by block in omvg_ba_create), so:
-//   schur_stage_kernel  : thread per observation (coalesced component-major loads), per-observation border / rhs
-//                         terms, writes H[obs] (144 B per observation, in observation order)
-//   schur_gather_kernel : warp per block (or per chunk of a long pair list), sums in registers in list order and
-//                         stores every element once: no atomics, and the same bits on every run (the landmarks
-//                         schur_kernel takes still add theirs with atomics)
-// KIU = intrinsic columns in use (3 pinhole .. 8 Brown): the generic 8-column body kept 16 Jacobian and 24 EtFi values
-// live per thread (162 registers, 3 CTAs per SM, 17 % of the warps active, 5x off its DRAM time).  An observation's
-// {H, E'F} goes through shared memory so that a warp writes its 32 H records (4.5 KB, contiguous) with full 256-byte
-// stores instead of 18 scattered 8-byte stores per lane, and the border terms read E'F back from there.
+// schur_kernel).  With E'E + D^2 = L L' per landmark p and
+//   H_t = L^-1 E'Fc_t (3 x 6) per observation,  G_p = L^-1 E'Fi_p (3 x KIU),  v_p = L^-1 E'b_p (3) per landmark,
+// every term of the reduced system is a plain sum:
+//   Scc(a,b) = [a == b] Fc'Fc - sum H_t' H_u     over the observation pairs (t, u) of one landmark, cam(t) = a, cam(u) = b
+//   Sci(q,c) = Fi'Fc(q,c) - sum G_p' H_t         over the observations t of pose c through group q
+//   rhs_c    = Fc'r(c)    - sum H_t' v_p         over the observations t of pose c
+//   Sii(q,q) = Fi'Fi(q)   - sum G_p' G_p,  rhs_q = Fi'r(q) - sum G_p' v_p    over the landmarks p of group q
+// (the same as (E'Fc)' (E'E + D^2)^-1 E'Fi etc. up to rounding).  So:
+//   schur_stage_kernel  : thread per observation (coalesced component-major loads), writes H[obs] (144 B per
+//                         observation, in observation order) and, from the thread of a landmark's first observation,
+//                         the landmark's {v_p, G_p} record
+//   schur_gather_kernel : the camera blocks, warp per block (or per chunk of a long pair list) over the co-visibility lists
+//   schur_border_kernel : CTA per pose over its observation list (Sci, rhs_c)
+//   corner_kernel / corner_final_kernel : the intrinsics corner, two-level over the landmarks
+// Each sums in list order and stores every element once: no atomics, and the same bits on every run (the landmarks
+// schur_kernel takes still add theirs with atomics).
+// An observation's H goes through shared memory so that a warp writes its 32 H records (4.5 KB, contiguous) with full
+// 256-byte stores instead of 18 scattered 8-byte stores per lane.
 // (H in camera order, so that a block reads two compact regions, was measured on config 2 on an H100 SXM at 700 W: the
 // gather time did not change and the scattered record stores cost the stage kernel 0.12 ms per LM step.)
 constexpr int HREC = 18;                             // doubles per H record
-constexpr int STAGE_LD = 37;                         // padded record stride in shared memory (conflict-free for both phases)
-constexpr int CORNER_REPS = 64;
+constexpr int STAGE_LD = 19;                         // padded record stride in shared memory (conflict-free per-lane writes)
+// doubles per {v_p, G_p} record: v (3), then G row-major (3 x KIU), padded to 16 bytes
+__host__ __device__ constexpr int gv_rec(int kiu) { return (3 + 3 * kiu + 1) & ~1; }
+__device__ __forceinline__ bool gather_point(const int *__restrict__ pt_start, const unsigned char *__restrict__ pt_single, int j) {
+  const int K = pt_start[j + 1] - pt_start[j];
+  return pt_single[j] != 0 && K > 0 && K <= 32;
+}
 template <int KIU>
-__global__ void __launch_bounds__(SCHUR_THREADS, 5) schur_stage_kernel(SchurArgs A, double *__restrict__ H, double *__restrict__ corner_rep) {
-  // The intrinsics corner (and its rhs) of group q0 is hit once per landmark: accumulate into CORNER_REPS replicas
-  // with native FP64 REDs (shared-memory double atomics are CAS loops: they cost 0.3 ms here) and fold them after.
+__global__ void __launch_bounds__(SCHUR_THREADS, 5) schur_stage_kernel(SchurArgs A, double *__restrict__ H, double *__restrict__ Gv) {
   __shared__ double rec_s[SCHUR_THREADS / 32][32 * STAGE_LD];
   const long long t = (long long)blockIdx.x * SCHUR_THREADS + threadIdx.x;
   const long long n = A.n;
-  const int nred_c = 6 * A.n_poses, ni8 = KI * A.n_intr;
-  const int q0 = A.obs_intr[0];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  double *s_ii = corner_rep + (size_t)(blockIdx.x % CORNER_REPS) * (KI * KI + KI);
   double *gs = rec_s[warp] + lane * STAGE_LD;
-  bool mine = t < n;
+  bool mine = false, first = false;
   int j = 0;
-  if (mine) { j = A.obs_pt[t]; const int K = A.pt_start[j + 1] - A.pt_start[j]; mine = A.pt_single[j] != 0 && K <= 32; }
+  if (t < n) { j = A.obs_pt[t]; const int s0 = A.pt_start[j], K = A.pt_start[j + 1] - s0; mine = A.pt_single[j] != 0 && K <= 32; first = t == s0; }
+  double *gv = Gv + (size_t)gv_rec(KIU) * j;
   if (mine) {
-    const int ct = A.obs_pose[t], qt = A.obs_intr[t];
-    double inv[9], ie[3], m[6], L[6];
+    double m[6], L[6];
     { const double *E = A.EtE + 6 * (size_t)j;
       const double d0 = A.lmD_pt[3 * j], d1 = A.lmD_pt[3 * j + 1], d2 = A.lmD_pt[3 * j + 2];
       m[0] = E[0] + d0 * d0; m[1] = E[1]; m[2] = E[2] + d1 * d1; m[3] = E[3]; m[4] = E[4]; m[5] = E[5] + d2 * d2; }
-    if (!inv3_spd(m, inv)) atomicExch(A.fail, 1);
-    chol3(m, L);
-    { const double *eb = A.Etb + 3 * (size_t)j;
-      #pragma unroll
-      for (int a = 0; a < 3; ++a) ie[a] = inv[a * 3] * eb[0] + inv[a * 3 + 1] * eb[1] + inv[a * 3 + 2] * eb[2]; }
-    const bool first = t == A.pt_start[j];
-    if (first) { for (int a = 0; a < 9; ++a) A.Einv[9 * (size_t)j + a] = inv[a]; }
+    chol3(m, L);                                     // (the pivots inv3_spd checks)
+    if (!(L[0] > 0.0 && L[2] > 0.0 && L[5] > 0.0) || !isfinite(L[0]) || !isfinite(L[2]) || !isfinite(L[5])) atomicExch(A.fail, 1);
+    const double r0 = 1.0 / L[0], r1 = 1.0 / L[2], r2 = 1.0 / L[5];
     double jc[12], jp[6];
     #pragma unroll
     for (int k = 0; k < 12; ++k) jc[k] = A.Jc[k * n + t];
     #pragma unroll
     for (int k = 0; k < 6; ++k) jp[k] = A.Jp[k * n + t];
-    // E'F (3 x 6) and H = L^-1 E'F (forward substitution, column by column), staged in shared memory
-    { double efc[18];
-      #pragma unroll
-      for (int a = 0; a < 3; ++a)
-        #pragma unroll
-        for (int c = 0; c < 6; ++c) efc[a * 6 + c] = jp[a] * jc[c] + jp[3 + a] * jc[6 + c];
-      const double r0 = 1.0 / L[0], r1 = 1.0 / L[2], r2 = 1.0 / L[5];
-      #pragma unroll
-      for (int c = 0; c < 6; ++c) {
-        const double h0 = efc[c] * r0, h1 = (efc[6 + c] - L[1] * h0) * r1, h2 = (efc[12 + c] - L[3] * h0 - L[4] * h1) * r2;
-        gs[c] = h0; gs[6 + c] = h1; gs[12 + c] = h2;
-      }
-      #pragma unroll
-      for (int k = 0; k < 18; ++k) gs[18 + k] = efc[k]; }
-    __syncwarp(__activemask());
-    const double *ef = gs + 18;
+    // H = L^-1 E'Fc (forward substitution, column by column), staged in shared memory
     #pragma unroll
-    for (int c = 0; c < 6; ++c) atomicAdd(&A.rhs[6 * ct + c], -(ef[c] * ie[0] + ef[6 + c] * ie[1] + ef[12 + c] * ie[2]));
-    double *sci_row0 = A.Sci + (size_t)(KI * qt) * nred_c + 6 * ct;
-    const double *fi = A.EtFi + (size_t)j * 3 * KI;
-    #pragma unroll
-    for (int a = 0; a < KIU; ++a) {
-      const double f0 = fi[a], f1 = fi[KI + a], f2 = fi[2 * KI + a];
-      const double ji0 = A.Ji[a * n + t], ji1 = A.Ji[(KI + a) * n + t];
-      if (f0 == 0.0 && f1 == 0.0 && f2 == 0.0 && ji0 == 0.0 && ji1 == 0.0) continue;   // constant parameter
-      const double g0 = inv[0] * f0 + inv[1] * f1 + inv[2] * f2, g1 = inv[3] * f0 + inv[4] * f1 + inv[5] * f2, g2 = inv[6] * f0 + inv[7] * f1 + inv[8] * f2;
+    for (int c = 0; c < 6; ++c) {
+      const double e0 = jp[0] * jc[c] + jp[3] * jc[6 + c], e1 = jp[1] * jc[c] + jp[4] * jc[6 + c], e2 = jp[2] * jc[c] + jp[5] * jc[6 + c];
+      const double h0 = e0 * r0, h1 = (e1 - L[1] * h0) * r1, h2 = (e2 - L[3] * h0 - L[4] * h1) * r2;
+      gs[c] = h0; gs[6 + c] = h1; gs[12 + c] = h2;
+    }
+    if (first) {                                     // once per landmark: Einv (back substitution), v_p and G_p
+      double inv[9];
+      inv3_spd(m, inv);
+      for (int a = 0; a < 9; ++a) A.Einv[9 * (size_t)j + a] = inv[a];
+      const double *eb = A.Etb + 3 * (size_t)j, *fi = A.EtFi + (size_t)j * 3 * KI;
+      { const double v0 = eb[0] * r0, v1 = (eb[1] - L[1] * v0) * r1, v2 = (eb[2] - L[3] * v0 - L[4] * v1) * r2;
+        gv[0] = v0; gv[1] = v1; gv[2] = v2; }
       #pragma unroll
-      for (int b = 0; b < 6; ++b)
-        atomicAdd(&sci_row0[(size_t)a * nred_c + b], ji0 * jc[b] + ji1 * jc[6 + b] - (g0 * ef[b] + g1 * ef[6 + b] + g2 * ef[12 + b]));
-      if (first) {
-        const double rv = -(f0 * ie[0] + f1 * ie[1] + f2 * ie[2]);
-        if (qt == q0) atomicAdd(&s_ii[KI * KI + a], rv); else atomicAdd(&A.rhs[nred_c + KI * qt + a], rv);
-        #pragma unroll
-        for (int b = 0; b < KIU; ++b) {
-          const double v = -(g0 * fi[b] + g1 * fi[KI + b] + g2 * fi[2 * KI + b]);
-          if (v == 0.0) continue;
-          if (qt == q0) atomicAdd(&s_ii[a * KI + b], v); else atomicAdd(&A.Sii[(size_t)(KI * qt + a) * ni8 + KI * qt + b], v);
-        }
+      for (int a = 0; a < KIU; ++a) {
+        const double g0 = fi[a] * r0, g1 = (fi[KI + a] - L[1] * g0) * r1, g2 = (fi[2 * KI + a] - L[3] * g0 - L[4] * g1) * r2;
+        gv[3 + a] = g0; gv[3 + KIU + a] = g1; gv[3 + 2 * KIU + a] = g2;
       }
     }
   } else {
     #pragma unroll
-    for (int k = 0; k < HREC; ++k) gs[k] = 0.0;       // (records of landmarks the general kernel handles are not read)
+    for (int k = 0; k < HREC; ++k) gs[k] = 0.0;       // a landmark of schur_kernel: zero H and {v, G}, so that the
+    if (first) {                                      // border and corner sums can run over it without a test
+      #pragma unroll
+      for (int k = 0; k < gv_rec(KIU); ++k) gv[k] = 0.0;
+    }
   }
   __syncwarp();
   // the warp's 32 records are contiguous in H: 18 coalesced 256-byte stores
@@ -948,24 +950,117 @@ __global__ void __launch_bounds__(SCHUR_THREADS, 5) schur_stage_kernel(SchurArgs
       for (int e = lane; e < HREC * (int)nrec; e += 32) dst[e] = rec_s[warp][(e / HREC) * STAGE_LD + e % HREC];
     } }
 }
-// folds the corner replicas of schur_stage_kernel into Sii / rhs of group q0 (fixed order)
-__global__ void corner_fold_kernel(const double *__restrict__ corner_rep, const int *__restrict__ obs_intr, int n_poses, int n_intr, double *__restrict__ Sii, double *__restrict__ rhs) {
-  const int e = threadIdx.x; if (e >= KI * KI + KI) return;
-  const int q0 = obs_intr[0], ni8 = KI * n_intr;
-  double v = 0; for (int rp2 = 0; rp2 < CORNER_REPS; ++rp2) v += corner_rep[(size_t)rp2 * (KI * KI + KI) + e];
-  if (v == 0.0) return;
-  if (e < KI * KI) atomicAdd(&Sii[(size_t)(KI * q0 + e / KI) * ni8 + KI * q0 + e % KI], v);
-  else atomicAdd(&rhs[6 * n_poses + KI * q0 + (e - KI * KI)], v);
+
+// Sci(q, c) and rhs_c, one CTA per pose c: the pose's list is ordered by intrinsic group, and every (pose, group) segment
+// stores its border block  FiFc[seg] - sum G_p' H_t;  rhs_c = g_cam(c) - sum H_t' v_p  over all segments.  Sums run in list
+// order per thread, then lane and warp order (cta_sum).  The records of schur_kernel's landmarks are zero (schur_stage_kernel),
+// so they add nothing here.  With constant structure (H null) the border is FiFc, rhs_c = g_cam(c), and the kernel also
+// stores the camera diagonal block Scc(c, c) = Fc'Fc (the other camera blocks are zero).
+struct BorderArgs {
+  const double *H, *Gv, *FiFc, *g_cam, *FtF; const int *cam_seg, *seg_start, *seg_intr, *cam_obs, *obs_pt;
+  int n_poses; double *Sci, *rhs, *Scc; Bsr bsr;
+};
+template <int KIU>
+__global__ void __launch_bounds__(CCS_THREADS) schur_border_kernel(BorderArgs B) {
+  __shared__ double sh[CCS_THREADS / 32 * KIU * 6];
+  constexpr int GW = gv_rec(KIU);
+  const int p = blockIdx.x, nred_c = 6 * B.n_poses;
+  double rc[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  for (int s = B.cam_seg[p]; s < B.cam_seg[p + 1]; ++s) {
+    double f[KIU * 6];
+    #pragma unroll
+    for (int k = 0; k < KIU * 6; ++k) f[k] = 0.0;
+    if (B.H)
+      for (int t = B.seg_start[s] + threadIdx.x; t < B.seg_start[s + 1]; t += CCS_THREADS) {
+        const int o = B.cam_obs[t], j = B.obs_pt[o];
+        double h[HREC], g[GW];
+        { const double2 *hp = reinterpret_cast<const double2 *>(B.H + HREC * (size_t)o);
+          #pragma unroll
+          for (int k = 0; k < HREC / 2; ++k) { const double2 v = __ldg(hp + k); h[2 * k] = v.x; h[2 * k + 1] = v.y; } }
+        { const double2 *gp = reinterpret_cast<const double2 *>(B.Gv + GW * (size_t)j);
+          #pragma unroll
+          for (int k = 0; k < GW / 2; ++k) { const double2 v = __ldg(gp + k); g[2 * k] = v.x; g[2 * k + 1] = v.y; } }
+        #pragma unroll
+        for (int c = 0; c < 6; ++c) rc[c] += h[c] * g[0] + h[6 + c] * g[1] + h[12 + c] * g[2];
+        #pragma unroll
+        for (int a = 0; a < KIU; ++a)
+          #pragma unroll
+          for (int c = 0; c < 6; ++c) f[6 * a + c] += g[3 + a] * h[c] + g[3 + KIU + a] * h[6 + c] + g[3 + 2 * KIU + a] * h[12 + c];
+      }
+    cta_sum<KIU * 6>(f, sh);
+    if (threadIdx.x < KIU * 6) {
+      const int a = threadIdx.x / 6, c = threadIdx.x % 6;
+      B.Sci[(size_t)(KI * B.seg_intr[s] + a) * nred_c + 6 * p + c] = B.FiFc[(size_t)s * KI * 6 + threadIdx.x] - sh[threadIdx.x];
+    }
+    __syncthreads();
+  }
+  cta_sum<6>(rc, sh);
+  if (threadIdx.x < 6) B.rhs[6 * p + threadIdx.x] = B.g_cam[6 * p + threadIdx.x] - sh[threadIdx.x];
+  if (B.Scc && threadIdx.x < 36) B.Scc[36 * (size_t)bsr_find(B.bsr, p, p) + threadIdx.x] = B.FtF[36 * (size_t)p + threadIdx.x];
+}
+
+// The intrinsics corner: per group q and chunk of landmarks, the partial sums of G_p' G_p (lower triangle) and G_p' v_p over
+// the landmarks of the co-visibility lists, in landmark order and then block order; part[q][chunk][ICS_W] as intr_colsum.
+constexpr int CORNER_THREADS = 256;
+template <int KIU>
+__global__ void __launch_bounds__(CORNER_THREADS) corner_kernel(const double *__restrict__ Gv, const int *__restrict__ pt_start, const unsigned char *__restrict__ pt_single,
+                                                               const int *__restrict__ obs_intr, int n_points, int chunks, double *__restrict__ part) {
+  __shared__ double sh[CORNER_THREADS / 32];
+  constexpr int NM = KIU * (KIU + 1) / 2, GW = gv_rec(KIU);
+  const int q = blockIdx.y, chunk = blockIdx.x;
+  double m[NM], g[KIU];
+  #pragma unroll
+  for (int k = 0; k < NM; ++k) m[k] = 0.0;
+  #pragma unroll
+  for (int k = 0; k < KIU; ++k) g[k] = 0.0;
+  const int per = (n_points + chunks - 1) / chunks, lo = per * chunk, hi = min(lo + per, n_points);
+  for (int j = lo + threadIdx.x; j < hi; j += CORNER_THREADS) {
+    if (!gather_point(pt_start, pt_single, j) || obs_intr[pt_start[j]] != q) continue;
+    double r[GW];
+    const double2 *gp = reinterpret_cast<const double2 *>(Gv + GW * (size_t)j);
+    #pragma unroll
+    for (int k = 0; k < GW / 2; ++k) { const double2 v = __ldg(gp + k); r[2 * k] = v.x; r[2 * k + 1] = v.y; }
+    const double *G0 = r + 3, *G1 = r + 3 + KIU, *G2 = r + 3 + 2 * KIU;
+    #pragma unroll
+    for (int k = 0; k < KIU; ++k) g[k] += G0[k] * r[0] + G1[k] * r[1] + G2[k] * r[2];
+    int t = 0;
+    #pragma unroll
+    for (int i = 0; i < KIU; ++i)
+      #pragma unroll
+      for (int k = 0; k <= i; ++k) m[t++] += G0[i] * G0[k] + G1[i] * G1[k] + G2[i] * G2[k];
+  }
+  double *dst = part + ((size_t)q * chunks + chunk) * ICS_W;
+  for (int e = threadIdx.x; e < ICS_W; e += CORNER_THREADS) dst[e] = 0.0;
+  __syncthreads();
+  int t = 0;
+  #pragma unroll
+  for (int i = 0; i < KIU; ++i)
+    #pragma unroll
+    for (int k = 0; k <= i; ++k) {
+      const double v = block_sum<CORNER_THREADS>(m[t++], sh);
+      if (threadIdx.x == 0) { dst[i * KI + k] = v; dst[k * KI + i] = v; }
+    }
+  #pragma unroll
+  for (int k = 0; k < KIU; ++k) { const double v = block_sum<CORNER_THREADS>(g[k], sh); if (threadIdx.x == 0) dst[64 + k] = v; }
+}
+// one CTA per (intrinsic group, element): Sii(q, q) = FiFi(q) - sum,  rhs_q = g_intr(q) - sum  over corner_kernel's chunks
+// (strided partial sums, then a fixed-order block reduction).  With part null (constant structure) the sums are zero.
+__global__ void __launch_bounds__(128) corner_final_kernel(const double *__restrict__ part, int chunks, int n_poses, int n_intr, const double *__restrict__ FiFi,
+                                                          const double *__restrict__ g_intr, double *__restrict__ Sii, double *__restrict__ rhs) {
+  __shared__ double sh[4];
+  const int q = blockIdx.x / 72, e = blockIdx.x % 72, ni8 = KI * n_intr;
+  double v = 0;
+  if (part) for (int c = threadIdx.x; c < chunks; c += 128) v += part[((size_t)q * chunks + c) * ICS_W + e];
+  v = block_sum<128>(v, sh);
+  if (threadIdx.x != 0) return;
+  if (e < 64) Sii[(size_t)(KI * q + e / KI) * ni8 + KI * q + e % KI] = FiFi[(size_t)q * 64 + e] - v;
+  else rhs[6 * n_poses + KI * q + (e - 64)] = g_intr[q * KI + (e - 64)] - v;
 }
 // ---- co-visibility lists of the camera blocks, built once per problem (omvg_ba_create).  For every landmark the
 // stage / gather pair takes (one intrinsic group, 1..32 observations) they hold the observation pairs (t, u) with
 // cam(u) >= cam(t), keyed by the BSR index of block (cam(t), cam(u)); a stable sort by key lists the pairs of every
 // upper and diagonal block in landmark order.  Outlier rejection and omvg_ba_remove_points only set weights to 0 and
 // make landmarks constant: their H records become zero and the lists stay valid without a rebuild.
-__device__ __forceinline__ bool gather_point(const int *__restrict__ pt_start, const unsigned char *__restrict__ pt_single, int j) {
-  const int K = pt_start[j + 1] - pt_start[j];
-  return pt_single[j] != 0 && K > 0 && K <= 32;
-}
 __global__ void pair_count_kernel(const int *__restrict__ pt_start, const unsigned char *__restrict__ pt_single, const int *__restrict__ obs_pose,
                                   int n_points, long long *__restrict__ count) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x; if (j >= n_points) return;
