@@ -16,6 +16,8 @@
 #include <limits>
 #include <memory>
 #include <chrono>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 using namespace omvg;
@@ -91,7 +93,52 @@ struct omvg_ba_ctx {
 
 namespace {
 
-#define LAUNCH_CHECK() OMVG_CUDA(cudaGetLastError())
+// Every kernel of the context is launched through launch() or launch_coop() (grid-wide barriers), which check the launch
+// and count it: the run summary reports the count as kernel_launches.
+template <typename... P, typename... A>
+int launch(omvg_ba_ctx *c, void (*k)(P...), dim3 grid, dim3 block, size_t smem, A &&...args) {
+  k<<<grid, block, smem, c->stream>>>(std::forward<A>(args)...);
+  OMVG_CUDA(cudaGetLastError());
+  ++c->launches; return OMVG_OK;
+}
+template <typename T> struct NoDeduce { using type = T; };
+template <typename... P>
+int launch_coop(omvg_ba_ctx *c, void (*k)(P...), dim3 grid, dim3 block, size_t smem, typename NoDeduce<P>::type... args) {
+  void *argv[] = {&args...};
+  OMVG_CUDA(cudaLaunchCooperativeKernel((void *)k, grid, block, argv, smem, c->stream));
+  ++c->launches; return OMVG_OK;
+}
+
+// Calls f(std::integral_constant<int, K>{}) for the intrinsic columns in use (kiu = max getParams() size over the groups,
+// at least 3): the kernels that take KIU as a template parameter are instantiated for K = 3, 4, 6, 7 and 8 only.
+template <typename F> int dispatch_kiu(int kiu, F &&f) {
+  switch (kiu) {
+    case 3: return f(std::integral_constant<int, 3>{});
+    case 4: return f(std::integral_constant<int, 4>{});
+    case 6: return f(std::integral_constant<int, 6>{});
+    case 7: return f(std::integral_constant<int, 7>{});
+    default: return f(std::integral_constant<int, 8>{});
+  }
+}
+
+// Phase clocks of a solver kernel (OMVG_BA_GJ_TIMING, OMVG_BA_DENSE_TIMING, OMVG_BA_PCG_TIMING): arm() hands the kernel a
+// zeroed buffer, or null when the switch is off; report() waits for the kernel and passes the phases in microseconds.
+struct DevTimer {
+  unsigned long long *p = nullptr;
+  int arm(omvg_ba_ctx *c, bool on) {
+    if (!on) return OMVG_OK;
+    if (!c->pcg_tim.p) { const int rc = c->pcg_tim.alloc(8); if (rc) return rc; }
+    p = c->pcg_tim.p; OMVG_CUDA(cudaMemsetAsync(p, 0, 64, c->stream)); return OMVG_OK;
+  }
+  template <typename F> int report(omvg_ba_ctx *c, F &&print) const {
+    if (!p) return OMVG_OK;
+    unsigned long long h[8]; OMVG_CUDA(cudaMemcpyAsync(h, p, sizeof h, cudaMemcpyDeviceToHost, c->stream)); OMVG_CUDA(cudaStreamSynchronize(c->stream));
+    double us[8]; for (int i = 0; i < 8; ++i) us[i] = h[i] * 1e-3;
+    print(us); return OMVG_OK;
+  }
+};
+
+int env_int(const char *name, int dflt) { const char *e = getenv(name); return e ? atoi(e) : dflt; }
 
 // OMVG_BA_TIMING=1: host wall-clock of the phases around the solve (where the end-to-end time goes)
 struct PhaseTimer {
@@ -130,7 +177,7 @@ template <typename T> int upload(DevBuf<T> &b, const T *h, size_t n, cudaStream_
 }
 
 int reduce_to(omvg_ba_ctx *c, const double *part, int n, int slot) {
-  reduce_partials_kernel<<<1, 1024, 0, c->stream>>>(part, n, c->scal.p + slot); LAUNCH_CHECK(); c->launches++; return OMVG_OK;
+  return launch(c, reduce_partials_kernel, 1, 1024, 0, part, n, c->scal.p + slot);
 }
 
 struct Masks { unsigned pose_mask; std::vector<unsigned> intr_mask; int pts_free; };
@@ -156,99 +203,109 @@ Masks make_masks(const omvg_ba_ctx *c, const omvg_ba_options *o) {
   return m;
 }
 
+// reduced-system solvers: dense_solve_kernel (L D L'), the explicit inverse, the block PCG (pcg5_kernel / pcg3_kernel) and
+// pcg_kernel on the whole system
+enum class Solver { DenseLdlt, DenseInverse, Pcg5, Pcg3, PcgWhole };
+constexpr size_t PCG3_SMEM = sizeof(Pcg2Smem) + 4 * PCG3_NCO_MAX * sizeof(double);
+
+// What a run does that the options, the masks and the structure built at create decide once: the reduced-system solver
+// and its launch parameters.  The environment switches are read here on every call.
+struct Plan {
+  Masks m;
+  Solver solver;
+  int nd = 0;                       // unknowns of the reduced system
+  int n_free_intr = 0;              // free intrinsic columns (right-hand sides of the border elimination - 1)
+  unsigned gen = 0; int nw = 0;     // gauge generators (PCG paths only)
+  bool use_coarse = false;          // aggregated coarse space: needs gauge freedom and two poses
+  Coarse co{};                      // (nw = nco = 0 without a coarse space: block-Jacobi alone)
+  int pcg_grid = 0;                 // CTAs of pcg3_kernel / pcg_kernel
+  int nb_cache = 0; size_t pcg5_smem = 0;   // neighbour S blocks pcg5 caches in shared memory, its dynamic shared memory
+  int coarse_every = 3;
+  bool gj_timing = false, dense_timing = false, pcg_timing = false;
+};
+
+// cam_prep_kernel for parameter set `which`, and the fields of the evaluation kernels' arguments that every caller shares
+int eval_prep(omvg_ba_ctx *c, int which, EvalArgs &A) {
+  A = EvalArgs{};
+  A.poses = c->pose[which].p; A.intr = c->intr[which].p; A.pts = c->pt[which].p; A.camR = c->camR[which].p; A.camdR = c->camdR.p; A.camrec = c->camrec[which].p;
+  A.obs_xy = c->obs_xy.p; A.intr_model = c->intr_model.p; A.obs_pose = c->obs_pose.p; A.obs_intr = c->obs_intr.p; A.obs_pt = c->obs_pt.p;
+  A.n_obs = c->no; A.cost_partial = c->part.p;
+  return launch(c, cam_prep_kernel, (c->nc + 127) / 128, 128, 0, c->pose[which].p, c->nc, c->camR[which].p, c->camdR.p, c->camrec[which].p);
+}
+
 int eval_cost(omvg_ba_ctx *c, const omvg_ba_options *o, int which, int slot) {
-  cam_prep_kernel<<<(c->nc + 127) / 128, 128, 0, c->stream>>>(c->pose[which].p, c->nc, c->camR[which].p, c->camdR.p, c->camrec[which].p); LAUNCH_CHECK();
   // NB: cam_prep overwrites camdR; the cost-only pass is always followed by a full evaluation before
   // camdR is read again (accepted step) or the current pose's camdR is not needed (J is materialised).
-  EvalArgs A{}; A.poses = c->pose[which].p; A.intr = c->intr[which].p; A.pts = c->pt[which].p; A.camR = c->camR[which].p; A.camdR = c->camdR.p; A.camrec = c->camrec[which].p;
-  A.obs_xy = c->obs_xy.p; A.intr_model = c->intr_model.p; A.obs_pose = c->obs_pose.p; A.obs_intr = c->obs_intr.p; A.obs_pt = c->obs_pt.p;
-  A.n_obs = c->no; A.use_loss = o->use_loss; A.huber_a = o->huber_a; A.cost_partial = c->part.p;
+  EvalArgs A; int rc = eval_prep(c, which, A); if (rc) return rc;
+  A.use_loss = o->use_loss; A.huber_a = o->huber_a;
   A.obs_w = c->obs_w.p; A.obs_flags = c->obs_flags.p; A.pt_fixed = c->pt_fixed.p;
-  if (c->has_ext) eval_kernel<false, 8, true><<<c->eval_grid, EVAL_THREADS, 0, c->stream>>>(A);
-  else eval_kernel<false, 8, false><<<c->eval_grid, EVAL_THREADS, 0, c->stream>>>(A);
-  LAUNCH_CHECK();
-  c->launches += 2;
+  if ((rc = launch(c, c->has_ext ? eval_kernel<false, 8, true> : eval_kernel<false, 8, false>, c->eval_grid, EVAL_THREADS, 0, A))) return rc;
   if (c->npri) {
     PriorArgs PA{}; PA.poses = c->pose[which].p; PA.camR = c->camR[which].p; PA.camdR = c->camdR.p; PA.prior_pose = c->prior_pose.p; PA.center = c->prior_center.p; PA.weight = c->prior_weight.p;
     PA.n = c->npri; PA.huber_a = c->prior_huber_a; PA.cost_out = c->part.p + c->eval_grid;
-    prior_eval_kernel<false><<<1, PRIOR_THREADS, 0, c->stream>>>(PA); LAUNCH_CHECK(); c->launches++;
+    if ((rc = launch(c, prior_eval_kernel<false>, 1, PRIOR_THREADS, 0, PA))) return rc;
   }
   return reduce_to(c, c->part.p, c->eval_grid + (c->npri ? 1 : 0), slot);
 }
 
-int colsums(omvg_ba_ctx *c) {
-  point_accum_kernel<<<(c->np + 127) / 128, 128, 0, c->stream>>>(c->Jp.p, c->Ji.p, c->r.p, c->pt_start.p, c->pt_single.p, c->np, c->no, c->kiu, c->EtE.p, c->Etb.p, c->EtFi.p, c->diag_pt.p); LAUNCH_CHECK();
-#define CCS(K) cam_colsum_kernel<K><<<c->nc, CCS_THREADS, 0, c->stream>>>(c->Jc.p, c->Ji.p, c->r.p, c->cam_seg.p, c->seg_start.p, c->cam_obs.p, c->nc, c->no, c->diag_cam.p, c->g_cam.p, c->FtF.p, c->FiFc.p)
-  switch (c->kiu) { case 3: CCS(3); break; case 4: CCS(4); break; case 6: CCS(6); break; case 7: CCS(7); break; default: CCS(8); break; }
-#undef CCS
-  LAUNCH_CHECK();
-  if (c->npri) { prior_accum_kernel<<<(c->npri + 127) / 128, 128, 0, c->stream>>>(c->JP.p, c->rP.p, c->prior_pose.p, c->npri, c->diag_cam.p, c->g_cam.p, c->FtF.p); LAUNCH_CHECK(); c->launches++; }
-  const int chunks = c->ics_chunks;
-  { const dim3 g(chunks, c->ni);
-    switch (c->kiu) {          // columns in use = max getParams() size over the intrinsic groups (3, 4, 6, 7 or 8)
-      case 3: intr_colsum_kernel<3><<<g, ICS_THREADS, 0, c->stream>>>(c->Ji.p, c->r.p, c->obs_intr.p, c->no, chunks, c->icol_part.p); break;
-      case 4: intr_colsum_kernel<4><<<g, ICS_THREADS, 0, c->stream>>>(c->Ji.p, c->r.p, c->obs_intr.p, c->no, chunks, c->icol_part.p); break;
-      case 6: intr_colsum_kernel<6><<<g, ICS_THREADS, 0, c->stream>>>(c->Ji.p, c->r.p, c->obs_intr.p, c->no, chunks, c->icol_part.p); break;
-      case 7: intr_colsum_kernel<7><<<g, ICS_THREADS, 0, c->stream>>>(c->Ji.p, c->r.p, c->obs_intr.p, c->no, chunks, c->icol_part.p); break;
-      default: intr_colsum_kernel<8><<<g, ICS_THREADS, 0, c->stream>>>(c->Ji.p, c->r.p, c->obs_intr.p, c->no, chunks, c->icol_part.p); break;
-    } }
-  LAUNCH_CHECK();
-  intr_colsum_final_kernel<<<c->ni * 72, 128, 0, c->stream>>>(c->icol_part.p, chunks, c->ni, c->diag_intr.p, c->g_intr.p, c->FiFi.p); LAUNCH_CHECK();
-  c->launches += 4; return OMVG_OK;
+// |r| in pixels (no weight, no loss) of every observation at the current parameters, into r (scratch between solves)
+int eval_pixel_norms(omvg_ba_ctx *c) {
+  EvalArgs A; const int rc = eval_prep(c, 0, A); if (rc) return rc;
+  A.use_loss = 0; A.rnorm = c->r.p;
+  return launch(c, eval_kernel<false, 8, false>, c->eval_grid, EVAL_THREADS, 0, A);
 }
 
-// full evaluation at parameter set `which`: cost, corrected r and J (scaled), column sums, gradient max
-int eval_jac(omvg_ba_ctx *c, const omvg_ba_options *o, const Masks &m, int which, bool &have_scale, bool time_it) {
-  cam_prep_kernel<<<(c->nc + 127) / 128, 128, 0, c->stream>>>(c->pose[which].p, c->nc, c->camR[which].p, c->camdR.p, c->camrec[which].p); LAUNCH_CHECK();
-  EvalArgs A{}; A.poses = c->pose[which].p; A.intr = c->intr[which].p; A.pts = c->pt[which].p; A.camR = c->camR[which].p; A.camdR = c->camdR.p; A.camrec = c->camrec[which].p;
-  A.obs_xy = c->obs_xy.p; A.intr_model = c->intr_model.p; A.obs_pose = c->obs_pose.p; A.obs_intr = c->obs_intr.p; A.obs_pt = c->obs_pt.p;
-  A.n_obs = c->no; A.use_loss = o->use_loss; A.huber_a = o->huber_a; A.r = c->r.p; A.Jp = c->Jp.p; A.Jc = c->Jc.p; A.Ji = c->Ji.p;
-  A.cost_partial = c->part.p; A.kiu = c->kiu; A.pose_mask = m.pose_mask; A.intr_mask = c->intr_mask.p; A.pts_free = m.pts_free;
+int colsums(omvg_ba_ctx *c) {
+  int rc;
+  if ((rc = launch(c, point_accum_kernel, (c->np + 127) / 128, 128, 0, c->Jp.p, c->Ji.p, c->r.p, c->pt_start.p, c->pt_single.p, c->np, c->no, c->kiu, c->EtE.p, c->Etb.p, c->EtFi.p, c->diag_pt.p))) return rc;
+  if ((rc = dispatch_kiu(c->kiu, [&](auto K) { return launch(c, cam_colsum_kernel<decltype(K)::value>, c->nc, CCS_THREADS, 0, c->Jc.p, c->Ji.p, c->r.p, c->cam_seg.p, c->seg_start.p, c->cam_obs.p,
+                                                            c->nc, c->no, c->diag_cam.p, c->g_cam.p, c->FtF.p, c->FiFc.p); }))) return rc;
+  if (c->npri && (rc = launch(c, prior_accum_kernel, (c->npri + 127) / 128, 128, 0, c->JP.p, c->rP.p, c->prior_pose.p, c->npri, c->diag_cam.p, c->g_cam.p, c->FtF.p))) return rc;
+  const int chunks = c->ics_chunks;
+  if ((rc = dispatch_kiu(c->kiu, [&](auto K) {
+         return launch(c, intr_colsum_kernel<decltype(K)::value>, dim3(chunks, c->ni), ICS_THREADS, 0, c->Ji.p, c->r.p, c->obs_intr.p, c->no, chunks, c->icol_part.p); }))) return rc;
+  return launch(c, intr_colsum_final_kernel, c->ni * 72, 128, 0, c->icol_part.p, chunks, c->ni, c->diag_intr.p, c->g_intr.p, c->FiFi.p);
+}
+
+// full evaluation at parameter set `which`: cost, corrected r and J (scaled), column sums, gradient max; the evaluation
+// kernel is timed (jacobian_ms of the summary)
+int eval_jac(omvg_ba_ctx *c, const omvg_ba_options *o, const Masks &m, int which, bool &have_scale) {
+  EvalArgs A; int rc = eval_prep(c, which, A); if (rc) return rc;
+  A.use_loss = o->use_loss; A.huber_a = o->huber_a; A.r = c->r.p; A.Jp = c->Jp.p; A.Jc = c->Jc.p; A.Ji = c->Ji.p;
+  A.kiu = c->kiu; A.pose_mask = m.pose_mask; A.intr_mask = c->intr_mask.p; A.pts_free = m.pts_free;
   A.obs_w = c->obs_w.p; A.obs_flags = c->obs_flags.p; A.pt_fixed = c->pt_fixed.p;
   if (have_scale) { A.sc_pt = c->sc_pt.p; A.sc_cam = c->sc_cam.p; A.sc_intr = c->sc_intr.p; }
-  if (time_it) OMVG_CUDA(cudaEventRecord(c->evj0, c->stream));
-  if (c->has_ext) eval_kernel<true, 4, true><<<c->eval_grid, EVAL_THREADS, 0, c->stream>>>(A);
-  else eval_kernel<true, 4, false><<<c->eval_grid, EVAL_THREADS, 0, c->stream>>>(A);
-  LAUNCH_CHECK();
-  if (time_it) OMVG_CUDA(cudaEventRecord(c->evj1, c->stream));
-  c->launches += 2;
+  OMVG_CUDA(cudaEventRecord(c->evj0, c->stream));
+  if ((rc = launch(c, c->has_ext ? eval_kernel<true, 4, true> : eval_kernel<true, 4, false>, c->eval_grid, EVAL_THREADS, 0, A))) return rc;
+  OMVG_CUDA(cudaEventRecord(c->evj1, c->stream));
   if (c->npri) {
     PriorArgs PA{}; PA.poses = c->pose[which].p; PA.camR = c->camR[which].p; PA.camdR = c->camdR.p; PA.prior_pose = c->prior_pose.p; PA.center = c->prior_center.p; PA.weight = c->prior_weight.p;
     PA.n = c->npri; PA.huber_a = c->prior_huber_a; PA.sc_cam = have_scale ? c->sc_cam.p : nullptr; PA.pose_mask = m.pose_mask; PA.rP = c->rP.p; PA.JP = c->JP.p; PA.cost_out = c->part.p + c->eval_grid;
-    prior_eval_kernel<true><<<1, PRIOR_THREADS, 0, c->stream>>>(PA); LAUNCH_CHECK(); c->launches++;
+    if ((rc = launch(c, prior_eval_kernel<true>, 1, PRIOR_THREADS, 0, PA))) return rc;
   }
-  int rc = reduce_to(c, c->part.p, c->eval_grid + (c->npri ? 1 : 0), S_COST); if (rc) return rc;
+  if ((rc = reduce_to(c, c->part.p, c->eval_grid + (c->npri ? 1 : 0), S_COST))) return rc;
   if (!have_scale) {        // iteration 0: Jacobi scaling from the unscaled J (trust_region_minimizer.cc:239-253)
     if ((rc = colsums(c))) return rc;
-    make_scale_kernel<<<(3 * c->np + 255) / 256, 256, 0, c->stream>>>(c->diag_pt.p, 3 * c->np, c->sc_pt.p); LAUNCH_CHECK();
-    make_scale_kernel<<<(6 * c->nc + 255) / 256, 256, 0, c->stream>>>(c->diag_cam.p, 6 * c->nc, c->sc_cam.p); LAUNCH_CHECK();
-    make_scale_kernel<<<(c->ni8 + 255) / 256, 256, 0, c->stream>>>(c->diag_intr.p, c->ni8, c->sc_intr.p); LAUNCH_CHECK();
-    scale_J_kernel<<<(unsigned)((c->no + 255) / 256), 256, 0, c->stream>>>(c->Jp.p, c->Jc.p, c->Ji.p, c->obs_pose.p, c->obs_intr.p, c->obs_pt.p, c->no, c->kiu,
-                                                                          c->sc_pt.p, c->sc_cam.p, c->sc_intr.p); LAUNCH_CHECK();
-    if (c->npri) { prior_scale_kernel<<<(18 * c->npri + 127) / 128, 128, 0, c->stream>>>(c->JP.p, c->prior_pose.p, c->sc_cam.p, c->npri); LAUNCH_CHECK(); c->launches++; }
-    c->launches += 4; have_scale = true;
+    if ((rc = launch(c, make_scale_kernel, (3 * c->np + 255) / 256, 256, 0, c->diag_pt.p, 3 * c->np, c->sc_pt.p)) ||
+        (rc = launch(c, make_scale_kernel, (6 * c->nc + 255) / 256, 256, 0, c->diag_cam.p, 6 * c->nc, c->sc_cam.p)) ||
+        (rc = launch(c, make_scale_kernel, (c->ni8 + 255) / 256, 256, 0, c->diag_intr.p, c->ni8, c->sc_intr.p)) ||
+        (rc = launch(c, scale_J_kernel, (unsigned)((c->no + 255) / 256), 256, 0, c->Jp.p, c->Jc.p, c->Ji.p, c->obs_pose.p, c->obs_intr.p, c->obs_pt.p, c->no, c->kiu,
+                     c->sc_pt.p, c->sc_cam.p, c->sc_intr.p))) return rc;
+    if (c->npri && (rc = launch(c, prior_scale_kernel, (18 * c->npri + 127) / 128, 128, 0, c->JP.p, c->prior_pose.p, c->sc_cam.p, c->npri))) return rc;
+    have_scale = true;
   }
   if ((rc = colsums(c))) return rc;
   // gradient max norm (unscaled): g = J_scaled' r / scale
   const int gb = 64;
   Vec3 GV{}; GV.s[0] = Vec3Seg{c->Etb.p, c->sc_pt.p, m.pts_free ? 3 * c->np : 0}; GV.s[1] = Vec3Seg{c->g_cam.p, c->sc_cam.p, 6 * c->nc}; GV.s[2] = Vec3Seg{c->g_intr.p, c->sc_intr.p, c->ni8};
-  grad_max3_kernel<<<dim3(gb, 3), 256, 0, c->stream>>>(GV, c->part2.p); LAUNCH_CHECK();     // part2[3][64], read back by read_scalars
-  c->launches += 1;
-  return OMVG_OK;
+  return launch(c, grad_max3_kernel, dim3(gb, 3), 256, 0, GV, c->part2.p);     // part2[3][64], read back by read_scalars
 }
 
 // gauge generators for the coarse space of the two-level preconditioner (needs camR/camdR of the CURRENT poses,
 // i.e. must run right after eval_jac and before any cost-only evaluation of a candidate)
-int make_gauge(omvg_ba_ctx *c, const Masks &m, int &nw) {
-  unsigned gen = 0;
-  if (m.pts_free) {
-    if ((m.pose_mask & 0x38u) == 0x38u) gen |= 0x0fu;       // translations + scale move t
-    if ((m.pose_mask & 0x07u) == 0x07u) gen |= 0x70u;       // rotations move the angle-axis
-  }
-  nw = __builtin_popcount(gen);
-  if (nw == 0) return OMVG_OK;
-  gauge_kernel<<<(c->nc + 63) / 64, 64, 0, c->stream>>>(c->pose[0].p, c->camR[0].p, c->camdR.p, c->sc_cam.p, m.pose_mask, c->nc, gen, nw, c->gW.p); LAUNCH_CHECK();
-  c->launches++; return OMVG_OK;
+int make_gauge(omvg_ba_ctx *c, const Plan &p) {
+  if (p.nw == 0) return OMVG_OK;
+  return launch(c, gauge_kernel, (c->nc + 63) / 64, 64, 0, c->pose[0].p, c->camR[0].p, c->camdR.p, c->sc_cam.p, p.m.pose_mask, c->nc, p.gen, p.nw, c->gW.p);
 }
 
 int read_scalars(omvg_ba_ctx *c) {
@@ -274,7 +331,7 @@ int build_pairs(omvg_ba_ctx *c, const std::vector<int> &hp, const std::vector<in
   DevBuf<long long> cnt, off; DevBuf<unsigned char> tmp, own;
   if ((rc = c->H.alloc(HREC * (size_t)c->no)) || (rc = cnt.alloc(c->np + 1)) || (rc = off.alloc(c->np + 1))) return rc;
   OMVG_CUDA(cudaMemsetAsync(cnt.p + c->np, 0, sizeof(long long), s));
-  pair_count_kernel<<<gp, 256, 0, s>>>(c->pt_start.p, c->pt_single.p, c->obs_pose.p, c->np, cnt.p); LAUNCH_CHECK();
+  if ((rc = launch(c, pair_count_kernel, gp, 256, 0, c->pt_start.p, c->pt_single.p, c->obs_pose.p, c->np, cnt.p))) return rc;
   { size_t tb = 0; OMVG_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt.p, off.p, c->np + 1, s));
     if ((rc = tmp.alloc(tb))) return rc;
     OMVG_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tb, cnt.p, off.p, c->np + 1, s)); }
@@ -292,11 +349,11 @@ int build_pairs(omvg_ba_ctx *c, const std::vector<int> &hp, const std::vector<in
     if (2 * kb + vb + tb > c->H.n * sizeof(double)) { if ((rc = own.alloc(2 * kb + vb + tb))) return rc; sc = own.p; }
     int *k0 = reinterpret_cast<int *>(sc), *k1 = reinterpret_cast<int *>(sc + kb);
     int2 *v1 = reinterpret_cast<int2 *>(sc + 2 * kb);
-    pair_emit_kernel<<<gp, 256, 0, s>>>(c->pt_start.p, c->pt_single.p, c->obs_pose.p, c->np, off.p, B, k0, c->pair.p); LAUNCH_CHECK();
+    if ((rc = launch(c, pair_emit_kernel, gp, 256, 0, c->pt_start.p, c->pt_single.p, c->obs_pose.p, c->np, off.p, B, k0, c->pair.p))) return rc;
     cub::DoubleBuffer<int> keys(k0, k1); cub::DoubleBuffer<int2> vals(c->pair.p, v1);
     OMVG_CUDA(cub::DeviceRadixSort::SortPairs(sc + 2 * kb + vb, tb, keys, vals, npair, 0, bits, s));
     if (npair && vals.Current() != c->pair.p) OMVG_CUDA(cudaMemcpyAsync(c->pair.p, vals.Current(), (size_t)npair * sizeof(int2), cudaMemcpyDeviceToDevice, s));
-    setup_starts_kernel<<<(unsigned)((npair + 256) / 256), 256, 0, s>>>(keys.Current(), npair, c->nnzb, c->pair_start.p); LAUNCH_CHECK(); }
+    if ((rc = launch(c, setup_starts_kernel, (unsigned)((npair + 256) / 256), 256, 0, keys.Current(), npair, c->nnzb, c->pair_start.p))) return rc; }
   std::vector<int> ps(c->nnzb + 1), first(c->nnzb + 1, 0), blk;
   OMVG_CUDA(cudaMemcpyAsync(ps.data(), c->pair_start.p, (c->nnzb + 1) * sizeof(int), cudaMemcpyDeviceToHost, s));
   OMVG_CUDA(cudaStreamSynchronize(s));
@@ -311,7 +368,6 @@ int build_pairs(omvg_ba_ctx *c, const std::vector<int> &hp, const std::vector<in
   if ((rc = c->ticket.alloc(c->nnzb)) || (rc = c->gpart.alloc(36 * (size_t)c->n_chunks))) return rc;
   OMVG_CUDA(cudaMemsetAsync(c->ticket.p, 0, c->nnzb * sizeof(int), s));
   OMVG_CUDA(cudaStreamSynchronize(s));
-  c->launches += 3;
   return OMVG_OK;
 }
 
@@ -326,9 +382,9 @@ int build_structure(omvg_ba_ctx *c) {
   std::vector<unsigned> diagbits((size_t)c->nc * c->words, 0u);
   for (int a = 0; a < c->nc; ++a) diagbits[(size_t)a * c->words + (a >> 5)] |= 1u << (a & 31);
   OMVG_CUDA(cudaMemcpyAsync(c->bitmap.p, diagbits.data(), diagbits.size() * 4, cudaMemcpyHostToDevice, c->stream));
-  if (c->no) { bitmap_mark_kernel<<<(unsigned)((c->no + 255) / 256), 256, 0, c->stream>>>(c->obs_pose.p, c->obs_pt.p, c->pt_start.p, c->no, c->bitmap.p, c->words); LAUNCH_CHECK(); }
+  if (c->no && (rc = launch(c, bitmap_mark_kernel, (unsigned)((c->no + 255) / 256), 256, 0, c->obs_pose.p, c->obs_pt.p, c->pt_start.p, c->no, c->bitmap.p, c->words))) return rc;
   DevBuf<int> rowcount; if ((rc = rowcount.alloc(c->nc))) return rc;
-  bitmap_rowcount_kernel<<<(c->nc + 127) / 128, 128, 0, c->stream>>>(c->bitmap.p, c->nc, c->words, c->wprefix.p, rowcount.p); LAUNCH_CHECK();
+  if ((rc = launch(c, bitmap_rowcount_kernel, (c->nc + 127) / 128, 128, 0, c->bitmap.p, c->nc, c->words, c->wprefix.p, rowcount.p))) return rc;
   std::vector<int> hc(c->nc), hp(c->nc + 1, 0);
   OMVG_CUDA(cudaMemcpyAsync(hc.data(), rowcount.p, c->nc * 4, cudaMemcpyDeviceToHost, c->stream));
   OMVG_CUDA(cudaStreamSynchronize(c->stream));
@@ -336,9 +392,8 @@ int build_structure(omvg_ba_ctx *c) {
   c->nnzb = hp[c->nc];
   OMVG_CUDA(cudaMemcpyAsync(c->rowptr.p, hp.data(), (c->nc + 1) * 4, cudaMemcpyHostToDevice, c->stream));
   if ((rc = c->cols.alloc(c->nnzb))) return rc;
-  bitmap_cols_kernel<<<(c->nc + 127) / 128, 128, 0, c->stream>>>(c->bitmap.p, c->rowptr.p, c->nc, c->words, c->cols.p); LAUNCH_CHECK();
+  if ((rc = launch(c, bitmap_cols_kernel, (c->nc + 127) / 128, 128, 0, c->bitmap.p, c->rowptr.p, c->nc, c->words, c->cols.p))) return rc;
   OMVG_CUDA(cudaStreamSynchronize(c->stream));
-  c->launches += 3;
   // ---- aggregates for the coarse space of the PCG preconditioner: greedy over the camera graph
   std::vector<int> hcols(c->nnzb), brow(c->nnzb);
   OMVG_CUDA(cudaMemcpy(hcols.data(), c->cols.p, (size_t)c->nnzb * 4, cudaMemcpyDeviceToHost));
@@ -432,6 +487,230 @@ int build_structure(omvg_ba_ctx *c) {
   return build_pairs(c, hp, hcols);
 }
 
+// The plan of a run (masks, solver, launch parameters, switches) and the kernel attributes it needs
+int plan_run(omvg_ba_ctx *c, const omvg_ba_options *O, Plan &p) {
+  p.m = make_masks(c, O);
+  p.nd = 6 * c->nc + c->ni8;
+  for (unsigned mm : p.m.intr_mask) p.n_free_intr += __builtin_popcount(mm);
+  p.coarse_every = std::max(1, env_int("OMVG_BA_COARSE_EVERY", 3));
+  p.gj_timing = getenv("OMVG_BA_GJ_TIMING") != nullptr;
+  p.dense_timing = getenv("OMVG_BA_DENSE_TIMING") != nullptr;
+  p.pcg_timing = getenv("OMVG_BA_PCG_TIMING") != nullptr;
+  // Small reduced systems are solved directly by one CTA (dense_solve_kernel: no gauge / coarse space / PCG), mid-size ones
+  // by an explicit inverse.  Beyond, up to 32 free intrinsic columns the block PCG (pcg5 / pcg3) eliminates the intrinsics
+  // border; with more, pcg_kernel iterates on the whole reduced system.  OMVG_BA_PCG1 forces pcg_kernel, so that tests can
+  // cross-check the two.
+  const int dense_max = std::min(DENSE_MAX, env_int("OMVG_BA_DENSE_MAX", DENSE_MAX));
+  const int dense2_max = std::min(1024, env_int("OMVG_BA_DENSE2_MAX", 640));
+  const bool block_pcg = p.n_free_intr <= MAXRHS - 1 && !getenv("OMVG_BA_PCG1");
+  // Small reduced systems are latency-bound on the grid-wide barriers of the PCG (4-5 us per iteration of pure
+  // synchronisation at 148 CTAs): up to `small_nc` poses ONE CTA runs the whole solve with block barriers instead.
+  // (measured: 0.70 vs 0.74 ms per LM iteration at 10 poses, but 0.99 vs 0.84 at 20: one CTA serialises the SpMV)
+  const int small_nc = env_int("OMVG_BA_PCG_SMALL", 12);
+  p.pcg_grid = (c->nc <= small_nc && block_pcg) ? 1 : c->n_sms;
+  if (p.nd <= dense_max) p.solver = Solver::DenseLdlt;
+  else if (p.nd <= dense2_max) p.solver = Solver::DenseInverse;
+  else {
+    if (p.m.pts_free) {                                       // gauge generators of the coarse space
+      if ((p.m.pose_mask & 0x38u) == 0x38u) p.gen |= 0x0fu;   // translations + scale move t
+      if ((p.m.pose_mask & 0x07u) == 0x07u) p.gen |= 0x70u;   // rotations move the angle-axis
+    }
+    p.nw = __builtin_popcount(p.gen);
+    p.use_coarse = p.nw > 0 && c->nc >= 2;
+    p.co = Coarse{c->agg_of.p, c->agg_start.p, c->agg_cams.p, c->ng, p.use_coarse ? p.nw : 0, p.use_coarse ? c->ng * p.nw : 0};
+    // pcg5: shared-memory resident, aggregate-owned (2 barriers + 2 L2 round trips per iteration).  Needs one CTA per
+    // aggregate, <= 4 right-hand sides (1 + free intrinsic columns) and aggregates of <= PCG5_MC cameras; else pcg3,
+    // on one CTA up to small_nc poses.
+    if (!block_pcg) p.solver = Solver::PcgWhole;
+    else if (p.pcg_grid > 1 && 1 + p.n_free_intr <= PCG5_NR && c->ng <= p.pcg_grid && c->agg_maxsize <= PCG5_MC && c->nb_max <= PCG5_NB && p.co.nco <= PCG3_NCO_MAX)
+      p.solver = Solver::Pcg5;
+    else p.solver = Solver::Pcg3;
+  }
+
+  // the per-observation kernels gather pose records (176 B x n_poses) and points through L1: give them all of it
+  for (auto k : {eval_kernel<true, 4, false>, eval_kernel<false, 8, false>, eval_kernel<true, 4, true>, eval_kernel<false, 8, true>})
+    OMVG_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, 0));
+  OMVG_CUDA(cudaFuncSetAttribute(pcg3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PCG3_SMEM));
+  if (p.solver == Solver::DenseLdlt) {
+    // The attribute is process-wide: set it to what any system size may need, never to this run's size, so that a
+    // smaller solve on another host thread cannot lower it under this launch.
+    static const int dense_smem_max = [] { int v = 0, dev = 0; cudaFuncAttributes fa{}; cudaGetDevice(&dev);
+      cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev); cudaFuncGetAttributes(&fa, dense_solve_kernel); return v - (int)fa.sharedSizeBytes; }();
+    OMVG_CUDA(cudaFuncSetAttribute(dense_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dense_smem_max));
+  }
+  if (p.solver == Solver::Pcg5) {           // all shared memory left over is a cache of neighbour S blocks
+    const size_t fixed = sizeof(Pcg5Red) + sizeof(Pcg5Smem) + (size_t)PCG5_NR * PCG3_NCO_MAX * sizeof(double) + (size_t)PCG5_NB * PCG5_PS * sizeof(double);
+    static const int smem_max = [] { int v = 0, dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev); return v; }();
+    p.nb_cache = (int)std::max<long long>(0, ((long long)smem_max - (long long)fixed - 2048) /   /* (static shared memory of the kernel + slack) */ (long long)(PCG5_BS * sizeof(double) + sizeof(unsigned short)));
+    p.pcg5_smem = fixed + (size_t)p.nb_cache * (PCG5_BS * sizeof(double) + sizeof(unsigned short)) + 16;
+    OMVG_CUDA(cudaFuncSetAttribute(pcg5_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.pcg5_smem));
+  }
+  if (p.solver == Solver::DenseInverse && !c->dA.p) {
+    int rc;
+    if ((rc = c->dA.alloc((size_t)p.nd * p.nd)) || (rc = c->dT.alloc(3 * (size_t)GJ_B * p.nd))) return rc;
+  }
+  if (!c->gj_grid) {                                        // as many co-resident CTAs as the tile count can use
+    int per_sm = 1; OMVG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, coarse_invert_kernel, 256, 0));
+    c->gj_grid = c->n_sms * std::max(1, std::min(per_sm, 2));
+  }
+  return OMVG_OK;
+}
+
+// LM diagonal (levenberg_marquardt_strategy.cc:75-87); diag_* always belong to the current J
+int lm_diagonal(omvg_ba_ctx *c, const omvg_ba_options *O, double radius) {
+  Diag3 DG{}; DG.s[0] = Diag3Seg{c->diag_pt.p, c->lmD_pt.p, 3 * c->np}; DG.s[1] = Diag3Seg{c->diag_cam.p, c->lmD_cam.p, 6 * c->nc}; DG.s[2] = Diag3Seg{c->diag_intr.p, c->lmD_intr.p, c->ni8};
+  const int nb = std::max(1, std::min(2 * c->n_sms, (3 * c->np + 255) / 256));
+  return launch(c, lm_diag3_kernel, dim3(nb, 3), 256, 0, DG, O->min_lm_diagonal, O->max_lm_diagonal, radius);
+}
+
+// Reduced camera system.  schur_stage writes H and the landmarks' {v, G}; schur_gather stores the camera blocks,
+// schur_border the intrinsics border and the camera right-hand side, corner / corner_final the intrinsics corner and its
+// right-hand side, all without atomics; then schur_kernel adds the landmarks outside the co-visibility lists (n_slow)
+// with atomics.  With constant structure the reduced system is its radius-independent part: Scc = diag(Fc'Fc) (stored
+// by schur_border), Sci = Fi'Fc, Sii = Fi'Fi.  finish_cam / finish_intr add the LM diagonal and invert the diagonal
+// blocks for the block-Jacobi preconditioner.
+int assemble_reduced(omvg_ba_ctx *c, const Plan &p) {
+  int rc;
+  const bool pts_free = p.m.pts_free;
+  { Zero4 Z{}; Z.p[0] = c->Scc.p; Z.n[0] = pts_free ? 0 : (long long)c->nnzb * 36;
+    Z.p[1] = c->Sci.p; Z.n[1] = c->n_slow > 0 ? (long long)c->Sci.n : 0; Z.p[2] = c->Sii.p; Z.n[2] = c->n_slow > 0 ? (long long)c->Sii.n : 0;
+    if (Z.n[0] || Z.n[1]) {
+      const int nb = (int)std::max<long long>(1, std::min<long long>(4 * c->n_sms, (std::max(Z.n[0], Z.n[1]) + 255) / 256));
+      if ((rc = launch(c, zero4_kernel, dim3(nb, 3), 256, 0, Z))) return rc;
+    } }
+  SchurArgs SA{}; SA.Jp = c->Jp.p; SA.Jc = c->Jc.p; SA.Ji = c->Ji.p; SA.EtE = c->EtE.p; SA.Etb = c->Etb.p; SA.EtFi = c->EtFi.p; SA.lmD_pt = c->lmD_pt.p; SA.pt_single = c->pt_single.p;
+  SA.obs_pose = c->obs_pose.p; SA.obs_intr = c->obs_intr.p; SA.obs_pt = c->obs_pt.p; SA.pt_start = c->pt_start.p; SA.n = c->no; SA.n_poses = c->nc; SA.n_intr = c->ni;
+  SA.kiu = c->kiu; SA.bsr = Bsr{c->bitmap.p, c->wprefix.p, c->rowptr.p, c->words}; SA.Scc = c->Scc.p; SA.Sci = c->Sci.p; SA.Sii = c->Sii.p; SA.rhs = c->rhs.p;
+  SA.Einv = c->Einv.p; SA.fail = c->fail.p;
+  const BorderArgs BA{pts_free ? c->H.p : nullptr, c->Gv.p, c->FiFc.p, c->g_cam.p, c->FtF.p, c->cam_seg.p, c->seg_start.p, c->seg_intr.p, c->cam_obs.p, c->obs_pt.p,
+                      c->nc, c->Sci.p, c->rhs.p, pts_free ? nullptr : c->Scc.p, SA.bsr};
+  const unsigned sg = (unsigned)((c->no + SCHUR_THREADS - 1) / SCHUR_THREADS);
+  if (pts_free) {
+    const GatherArgs G{c->H.p, c->FtF.p, c->pair.p, c->pair_start.p, c->chunk_blk.p, c->chunk_first.p, c->brow.p, c->cols.p, SA.bsr, c->Scc.p, c->gpart.p, c->ticket.p, c->n_chunks};
+    if ((rc = dispatch_kiu(c->kiu, [&](auto K) { return launch(c, schur_stage_kernel<decltype(K)::value>, sg, SCHUR_THREADS, 0, SA, c->H.p, c->Gv.p); })) ||
+        (rc = launch(c, schur_gather_kernel, (c->n_chunks + 7) / 8, 256, 0, G)) ||
+        (rc = dispatch_kiu(c->kiu, [&](auto K) {
+           return launch(c, corner_kernel<decltype(K)::value>, dim3(c->corner_chunks, c->ni), CORNER_THREADS, 0, c->Gv.p, c->pt_start.p, c->pt_single.p, c->obs_intr.p, c->np,
+                         c->corner_chunks, c->corner_part.p); }))) return rc;
+  }
+  if ((rc = dispatch_kiu(c->kiu, [&](auto K) { return launch(c, schur_border_kernel<decltype(K)::value>, c->nc, CCS_THREADS, 0, BA); })) ||
+      (rc = launch(c, corner_final_kernel, c->ni * 72, 128, 0, pts_free ? c->corner_part.p : nullptr, c->corner_chunks, c->nc, c->ni, c->FiFi.p, c->g_intr.p, c->Sii.p, c->rhs.p))) return rc;
+  if (pts_free && c->n_slow > 0) {
+    if ((rc = launch(c, schur_kernel, sg, SCHUR_THREADS, 0, SA)) ||
+        (rc = launch(c, mirror_kernel, (c->nc * 32 + 255) / 256, 256, 0, c->Scc.p, SA.bsr, c->cols.p, c->nc))) return rc;
+  }
+  const bool dense = p.solver == Solver::DenseLdlt || p.solver == Solver::DenseInverse;
+  if ((rc = launch(c, finish_cam_kernel, (c->nc + 63) / 64, 64, 0, c->Scc.p, SA.bsr, c->lmD_cam.p, p.m.pose_mask, c->nc, c->Minv_c.p, c->fail.p, dense ? 0 : 1))) return rc;
+  return launch(c, finish_intr_kernel, 1, 256, 0, c->Sii.p, c->lmD_intr.p, c->intr_mask.p, c->ni8, c->Minv_i.p, c->work_i.p, c->fail.p, p.solver == Solver::PcgWhole ? 1 : 0);
+}
+
+// Coarse operator of the two-level preconditioner (aggregated gauge space), shared by all PCG kernels.
+// It is only a preconditioner: a slightly stale E^-1 (previous LM step, radius/3) costs a few extra PCG
+// iterations (measured 38->40, 42->49, 43->43) but saves its O(nco^3) setup, so it is refreshed every
+// `coarse_every` LM steps (measured at 1000 cameras, ms per solve: every step 17.9, 2: 16.0, 3: 15.2, 5: 15.9),
+// or earlier if the last solve needed 1.5x the iterations seen right after a refresh.
+struct CoarseState {
+  int age = -1; double last_its = 0, fresh_its = 1e30; bool fresh_pending = false;
+  void solved(double its) { last_its = its; if (fresh_pending) { fresh_its = its; fresh_pending = false; } }
+};
+int refresh_coarse(omvg_ba_ctx *c, const Plan &p, CoarseState &cs) {
+  if (!p.use_coarse) return OMVG_OK;
+  const bool refresh = cs.age < 0 || cs.age >= p.coarse_every || cs.last_its > 1.5 * cs.fresh_its + 5;
+  if (refresh) { cs.age = 0; cs.fresh_pending = true; }
+  ++cs.age;
+  if (!refresh) return OMVG_OK;
+  const int nco = p.co.nco;
+  int rc;
+  OMVG_CUDA(cudaMemsetAsync(c->cE.p, 0, (size_t)nco * nco * sizeof(double), c->stream));
+  if ((rc = launch(c, coarse_assemble_kernel, (c->nnzb + 127) / 128, 128, 0, c->Scc.p, c->brow.p, c->cols.p, c->nnzb, c->gW.p, c->nc, p.co, c->cE.p))) return rc;
+  // blocked Gauss-Jordan, in place: cE becomes E^-1
+  DevTimer T; if ((rc = T.arm(c, p.gj_timing))) return rc;
+  const int mt = (nco + CT - 1) / CT;                     // no more CTAs than 64x64 tiles: a small coarse space pays for fewer barrier participants
+  const int gj = std::max(1, std::min(c->gj_grid, mt * mt));
+  if ((rc = launch_coop(c, coarse_invert_kernel, gj, 256, 0, c->cE.p, nco, c->cT.p, c->fail.p, T.p))) return rc;
+  return T.report(c, [&](const double *us) {
+    fprintf(stderr, "[omvg_ba gj timing] us: pivot inverse %.1f slices %.1f sync %.1f tiles %.1f sync %.1f (n %d, %d CTAs)\n", us[0], us[1], us[2], us[3], us[4], nco, c->gj_grid); });
+}
+
+// S z = rhs by the plan's solver; the iteration count goes to S_PCG_IT
+int solve_reduced(omvg_ba_ctx *c, const omvg_ba_options *O, const Plan &p) {
+  int rc;
+  switch (p.solver) {
+    case Solver::DenseLdlt: {
+      const size_t dsm = ((size_t)p.nd * (p.nd + 1) / 2 + (3 + DENSE_NB) * (size_t)p.nd) * sizeof(double);
+      DevTimer T; if ((rc = T.arm(c, p.dense_timing))) return rc;
+      if ((rc = launch(c, dense_solve_kernel, 1, 1024, dsm, c->Scc.p, c->rowptr.p, c->cols.p, c->Sci.p, c->Sii.p, c->rhs.p, c->nc, c->ni8, c->z.p, c->fail.p,
+                       c->scal.p + S_PCG_IT, T.p))) return rc;
+      return T.report(c, [&](const double *us) {
+        fprintf(stderr, "[omvg_ba dense timing] n %d us: assemble %.1f factor %.1f backward %.1f\n", p.nd, us[0], us[1], us[2]); });
+    }
+    case Solver::DenseInverse: {
+      const int nd = p.nd, mt = (nd + CT - 1) / CT;
+      OMVG_CUDA(cudaMemsetAsync(c->dA.p, 0, (size_t)nd * nd * sizeof(double), c->stream));
+      if ((rc = launch(c, dense_assemble_kernel, std::max(1, std::min(4 * c->n_sms, (36 * c->nnzb + 255) / 256)), 256, 0, c->Scc.p, c->brow.p, c->cols.p, c->nnzb,
+                       c->Sci.p, c->Sii.p, c->nc, c->ni8, c->dA.p)) ||
+          (rc = launch_coop(c, coarse_invert_kernel, std::max(1, std::min(c->gj_grid, mt * mt)), 256, 0, c->dA.p, nd, c->dT.p, c->fail.p, nullptr))) return rc;
+      return launch(c, dense_apply_kernel, (nd * 32 + 255) / 256, 256, 0, c->dA.p, c->rhs.p, nd, c->z.p, c->scal.p + S_PCG_IT);
+    }
+    case Solver::Pcg5:
+    case Solver::Pcg3: {
+      Pcg2Args P2{}; P2.Scc = c->Scc.p; P2.rowptr = c->rowptr.p; P2.cols = c->cols.p; P2.Sci = c->Sci.p; P2.Sii = c->Sii.p; P2.rhs = c->rhs.p; P2.Minv_c = c->Minv_c.p;
+      P2.W = c->gW.p; P2.intr_mask = c->intr_mask.p; P2.n_poses = c->nc; P2.ni8 = c->ni8; P2.X = c->bX.p; P2.Rv = c->bR.p; P2.Pv = c->bP.p; P2.Wv = c->bW.p; P2.Zv = c->bZ.p;
+      P2.part = c->pcg2_part.p; P2.z = c->z.p; P2.tol = O->pcg_tolerance; P2.max_iter = O->pcg_max_iterations; P2.out = c->scal.p + S_PCG_IT;
+      DevTimer T; if ((rc = T.arm(c, p.pcg_timing))) return rc;
+      Pcg3Args P3{}; P3.base = P2; P3.C = p.co; P3.Einv = c->cE.p; P3.Cv = c->cCv.p; P3.Yv = c->cYv.p; P3.Pv2 = c->bP2.p; P3.tim = T.p;
+      if (p.solver == Solver::Pcg3) {
+        if ((rc = launch_coop(c, pcg3_kernel, p.pcg_grid, PCG2_THREADS, PCG3_SMEM, P3))) return rc;
+        return T.report(c, [](const double *us) {
+          fprintf(stderr, "[omvg_ba pcg timing] us: coarse (stage %.1f rows %.1f sync %.1f) z %.1f spmv %.1f update %.1f tail %.1f border %.1f\n", us[6], us[7], us[0], us[1], us[2], us[3], us[4], us[5]); });
+      }
+      // one CTA per aggregate and no more: idle CTAs would only add participants to the two barriers of every iteration
+      if ((rc = launch_coop(c, pcg5_kernel, std::max(1, c->ng), PCG2_THREADS, p.pcg5_smem, P3, c->cCv2.p, c->cAW.p, p.nb_cache, c->nb_start.p, c->nb_list.p, c->blk_lcol.p))) return rc;
+      return T.report(c, [&](const double *us) {
+        fprintf(stderr, "[omvg_ba pcg5 timing] us: A wait-AW %.1f y %.1f local %.1f reduce %.1f | B gather %.1f rows %.1f publish %.1f reduce %.1f (cache %d blocks)\n", us[0], us[1], us[2], us[3], us[6], us[7], us[4], us[5], p.nb_cache); });
+    }
+    case Solver::PcgWhole: {
+      // more than 32 free intrinsic columns (e.g. one intrinsic group per image): PCG on the whole reduced system
+      // [Scc Sci'; Sci Sii] with the same aggregated coarse space on the camera rows and block-Jacobi on the intrinsics
+      PcgArgs PA{}; PA.Scc = c->Scc.p; PA.rowptr = c->rowptr.p; PA.cols = c->cols.p; PA.Sci = c->Sci.p; PA.Sii = c->Sii.p; PA.rhs = c->rhs.p; PA.Minv_c = c->Minv_c.p; PA.Minv_i = c->Minv_i.p;
+      PA.n_poses = c->nc; PA.ni8 = c->ni8; PA.z = c->z.p; PA.res = c->res.p; PA.p = c->pvec.p; PA.w = c->w.p; PA.zeta = c->zeta.p; PA.part = c->pcg_part.p;
+      PA.tol = O->pcg_tolerance; PA.max_iter = O->pcg_max_iterations; PA.out = c->scal.p + S_PCG_IT;
+      if (p.use_coarse) { PA.W = c->gW.p; PA.C = p.co; PA.Einv = c->cE.p; PA.Cv = c->cCv.p; PA.Yv = c->cYv.p; }
+      return launch_coop(c, pcg_kernel, p.pcg_grid, 256, 0, PA);
+    }
+  }
+  return fail(OMVG_E_ARG, "no reduced-system solver");
+}
+
+// back substitution, step = -y (constant structure: the landmark step stays zero), and the model cost change
+int back_substitute(omvg_ba_ctx *c, const Plan &p) {
+  int rc;
+  OMVG_CUDA(cudaMemsetAsync(c->step_pt.p, 0, 3 * (size_t)c->np * sizeof(double), c->stream));
+  if (p.m.pts_free) {
+    if ((rc = launch(c, backsub_obs_kernel, (unsigned)((c->no + 255) / 256), 256, 0, c->Jp.p, c->Jc.p, c->Ji.p, c->obs_pose.p, c->obs_intr.p, c->obs_pt.p, c->nc, c->no, c->kiu,
+                     c->z.p, c->step_pt.p)) ||
+        (rc = launch(c, backsub_point_kernel, (c->np + 255) / 256, 256, 0, c->Etb.p, c->Einv.p, c->pt_start.p, c->np, p.m.pts_free, c->step_pt.p))) return rc;
+  }
+  if ((rc = launch(c, negate_kernel, (c->nred + 255) / 256, 256, 0, c->z.p, c->nred, c->step_red.p)) ||
+      (rc = launch(c, model_kernel, c->eval_blocks, MODEL_THREADS, 0, c->r.p, c->Jp.p, c->Jc.p, c->Ji.p, c->obs_pose.p, c->obs_intr.p, c->obs_pt.p, c->no, c->nc, c->kiu,
+                   c->step_pt.p, c->step_red.p, c->part.p))) return rc;
+  if (c->npri && (rc = launch(c, prior_model_kernel, 1, PRIOR_THREADS, 0, c->JP.p, c->rP.p, c->prior_pose.p, c->npri, c->step_red.p, c->part.p + c->eval_blocks))) return rc;
+  return reduce_to(c, c->part.p, c->eval_blocks + (c->npri ? 1 : 0), S_MODEL);
+}
+
+// candidate = Plus(x, step * scale) for the three parameter blocks; |step|^2 and |x|^2 into S_STEP2_* / S_X2_*
+int update_all(omvg_ba_ctx *c, const Masks &m) {
+  const int ub = 64;
+  Upd3 U{};
+  U.s[0] = UpdSeg{c->pt[0].p, c->step_pt.p, c->sc_pt.p, 3 * c->np, 3, m.pts_free ? 7u : 0u, m.pts_free ? c->pt_mask.p : nullptr, c->pt[1].p};
+  U.s[1] = UpdSeg{c->pose[0].p, c->step_red.p, c->sc_cam.p, 6 * c->nc, 6, m.pose_mask, nullptr, c->pose[1].p};
+  U.s[2] = UpdSeg{c->intr[0].p, c->step_red.p + 6 * c->nc, c->sc_intr.p, c->ni8, KI, 0u, c->intr_mask.p, c->intr[1].p};
+  static_assert(S_STEP2_POSE == S_STEP2_PT + 1 && S_STEP2_INTR == S_STEP2_PT + 2 && S_X2_PT == S_STEP2_PT + 3 && S_X2_POSE == S_STEP2_PT + 4 && S_X2_INTR == S_STEP2_PT + 5, "slot order");
+  int rc;
+  if ((rc = launch(c, update3_kernel, dim3(ub, 3), 256, 0, U, c->part3.p))) return rc;
+  return launch(c, reduce_multi_kernel, 6, 1024, 0, c->part3.p, ub, c->scal.p + S_STEP2_PT);
+}
+
 }  // namespace
 
 extern "C" {
@@ -484,7 +763,7 @@ int omvg_ba_create(omvg_ba_ctx **out, int device, const omvg_ba_problem *P) {
     c->stream = r.stream; c->stream2 = r.stream2; c->ev0 = r.ev[0]; c->ev1 = r.ev[1]; c->evj0 = r.ev[2]; c->evj1 = r.ev[3]; c->ev_up = r.ev[4]; c->h_scal = r.h_scal; }
   c->nc = P->n_poses; c->ni = P->n_intrinsics; c->np = P->n_points; c->nv = P->n_views; c->no = P->n_obs;
   c->ni8 = KI * c->ni; c->nred = 6 * c->nc + c->ni8; c->eval_blocks = (int)std::max<long long>(1, (c->no + EVAL_THREADS - 1) / EVAL_THREADS);
-  c->eval_grid = std::min(c->eval_blocks, c->n_sms * (getenv("OMVG_BA_EVAL_WAVES") ? atoi(getenv("OMVG_BA_EVAL_WAVES")) : 4));   // persistent grid-stride evaluation
+  c->eval_grid = std::min(c->eval_blocks, c->n_sms * env_int("OMVG_BA_EVAL_WAVES", 4));   // persistent grid-stride evaluation
   tm.lap("stream+events+pinned");
   c->h_intr_model.assign(P->intr_model, P->intr_model + c->ni);
   c->kiu = 3; for (int q = 0; q < c->ni; ++q) c->kiu = std::max(c->kiu, model_nparams(P->intr_model[q]));   // (>= 3: the column-sum kernels are instantiated for 3, 4, 6, 7, 8)
@@ -515,7 +794,7 @@ int omvg_ba_create(omvg_ba_ctx **out, int device, const omvg_ba_problem *P) {
     if ((rc = c->pt_start.alloc(c->np + 1)) || (rc = c->cam_start.alloc(c->nc + 1)) || (rc = c->cam_obs.alloc(no)) || (rc = c->pt_single.alloc(c->np))) return rc;
     const int h_big = 0x7fffffff; OMVG_CUDA(cudaMemcpyAsync(bad.p, &h_big, sizeof(int), cudaMemcpyHostToDevice, s));
     const unsigned gb = (unsigned)((no + 255) / 256);
-    setup_check_kernel<<<gb, 256, 0, s>>>(raw_view.p, raw_point.p, no, c->nv, c->np, keys.p, iota.p, bad.p); LAUNCH_CHECK();
+    if ((rc = launch(c, setup_check_kernel, gb, 256, 0, raw_view.p, raw_point.p, no, c->nv, c->np, keys.p, iota.p, bad.p))) return rc;
     int pbits = 1; while ((1ll << pbits) < c->np) ++pbits;
     int cbits = 1; while ((1ll << cbits) < c->nc) ++cbits;
     int ibits = 1; while ((1ll << ibits) < c->ni) ++ibits;
@@ -527,37 +806,36 @@ int omvg_ba_create(omvg_ba_ctx **out, int device, const omvg_ba_problem *P) {
     if ((rc = cubtmp.alloc(std::max(std::max(tb1, tb2), std::max(tb3, tb4))))) return rc;
     size_t tb = cubtmp.n;
     OMVG_CUDA(cub::DeviceRadixSort::SortPairs(cubtmp.p, tb, keys.p, c->obs_pt.p, iota.p, c->d_perm.p, (int)no, 0, pbits, s));
-    setup_gather_kernel<<<gb, 256, 0, s>>>(c->d_perm.p, raw_view.p, d_view_pose.p, d_view_intr.p, nullptr, nullptr, nullptr, no, c->nv,
-                                           c->obs_pose.p, c->obs_intr.p, nullptr, nullptr, nullptr, iota.p); LAUNCH_CHECK();
-    setup_starts_kernel<<<(unsigned)((no + 256) / 256), 256, 0, s>>>(c->obs_pt.p, no, c->np, c->pt_start.p); LAUNCH_CHECK();
+    if ((rc = launch(c, setup_gather_kernel, gb, 256, 0, c->d_perm.p, raw_view.p, d_view_pose.p, d_view_intr.p, nullptr, nullptr, nullptr, no, c->nv,
+                     c->obs_pose.p, c->obs_intr.p, nullptr, nullptr, nullptr, iota.p))) return rc;
+    if ((rc = launch(c, setup_starts_kernel, (unsigned)((no + 256) / 256), 256, 0, c->obs_pt.p, no, c->np, c->pt_start.p))) return rc;
     // the per-pose lists: landmark order within each intrinsic group of the pose (with several groups a stable sort by
     // group comes first), cut into (pose, group) segments: the blocks of the intrinsics border
     const int *pose_key = c->obs_pose.p, *pose_val = iota.p;
     if (c->ni > 1) {
       tb = cubtmp.n;
       OMVG_CUDA(cub::DeviceRadixSort::SortPairs(cubtmp.p, tb, c->obs_intr.p, keys.p, iota.p, perm1.p, (int)no, 0, ibits, s));
-      setup_permute_kernel<<<gb, 256, 0, s>>>(perm1.p, c->obs_pose.p, no, keys.p); LAUNCH_CHECK();
-      pose_key = keys.p; pose_val = perm1.p; c->launches++;
+      if ((rc = launch(c, setup_permute_kernel, gb, 256, 0, perm1.p, c->obs_pose.p, no, keys.p))) return rc;
+      pose_key = keys.p; pose_val = perm1.p;
     }
     tb = cubtmp.n;
     OMVG_CUDA(cub::DeviceRadixSort::SortPairs(cubtmp.p, tb, pose_key, keys2.p, pose_val, c->cam_obs.p, (int)no, 0, cbits, s));
-    setup_starts_kernel<<<(unsigned)((no + 256) / 256), 256, 0, s>>>(keys2.p, no, c->nc, c->cam_start.p); LAUNCH_CHECK();
-    setup_seg_flag_kernel<<<(unsigned)((no + 256) / 256), 256, 0, s>>>(keys2.p, c->cam_obs.p, c->obs_intr.p, no, flag.p); LAUNCH_CHECK();
+    if ((rc = launch(c, setup_starts_kernel, (unsigned)((no + 256) / 256), 256, 0, keys2.p, no, c->nc, c->cam_start.p)) ||
+        (rc = launch(c, setup_seg_flag_kernel, (unsigned)((no + 256) / 256), 256, 0, keys2.p, c->cam_obs.p, c->obs_intr.p, no, flag.p))) return rc;
     tb = cubtmp.n;
     OMVG_CUDA(cub::DeviceScan::ExclusiveSum(cubtmp.p, tb, flag.p, seg_id.p, no + 1, s));
     DevBuf<int> slow; if ((rc = slow.alloc(1))) return rc;
     OMVG_CUDA(cudaMemsetAsync(slow.p, 0, sizeof(int), s));
-    setup_single_kernel<<<(c->np + 255) / 256, 256, 0, s>>>(c->obs_intr.p, c->pt_start.p, c->np, c->pt_single.p, slow.p); LAUNCH_CHECK();
+    if ((rc = launch(c, setup_single_kernel, (c->np + 255) / 256, 256, 0, c->obs_intr.p, c->pt_start.p, c->np, c->pt_single.p, slow.p))) return rc;
     int h_bad = 0; OMVG_CUDA(cudaMemcpyAsync(&h_bad, bad.p, sizeof(int), cudaMemcpyDeviceToHost, s));
     OMVG_CUDA(cudaMemcpyAsync(&c->n_slow, slow.p, sizeof(int), cudaMemcpyDeviceToHost, s));
     OMVG_CUDA(cudaMemcpyAsync(&c->nseg, seg_id.p + no, sizeof(int), cudaMemcpyDeviceToHost, s));
     OMVG_CUDA(cudaStreamSynchronize(s));
     if (h_bad != h_big) return fail(OMVG_E_ARG, "observation %d out of range", h_bad);
     if ((rc = c->seg_start.alloc(c->nseg + 1)) || (rc = c->seg_intr.alloc(c->nseg)) || (rc = c->cam_seg.alloc(c->nc + 1))) return rc;
-    setup_seg_emit_kernel<<<(unsigned)((std::max<long long>(no, c->nc) + 256) / 256), 256, 0, s>>>(flag.p, seg_id.p, c->cam_obs.p, c->obs_intr.p, c->cam_start.p, no, c->nc,
-                                                                                               c->seg_start.p, c->seg_intr.p, c->cam_seg.p); LAUNCH_CHECK();
+    if ((rc = launch(c, setup_seg_emit_kernel, (unsigned)((std::max<long long>(no, c->nc) + 256) / 256), 256, 0, flag.p, seg_id.p, c->cam_obs.p, c->obs_intr.p, c->cam_start.p,
+                     no, c->nc, c->seg_start.p, c->seg_intr.p, c->cam_seg.p))) return rc;
     OMVG_CUDA(cudaStreamSynchronize(s));                      // the temporaries above are released at the end of this scope
-    c->launches += 11;
     tm.lap("device sort / lists");
   }
   if (P->point_fixed) {
@@ -601,9 +879,8 @@ int omvg_ba_create(omvg_ba_ctx **out, int device, const omvg_ba_problem *P) {
   if ((rc = build_structure(c))) return rc;
   tm.lap("structure");
   OMVG_CUDA(cudaStreamWaitEvent(s, c->ev_up, 0));
-  setup_gather_xy_kernel<<<(unsigned)((no + 255) / 256), 256, 0, s>>>(c->d_perm.p, reinterpret_cast<const double2 *>(raw_xy.p), raw_w.p, raw_fl.p, no,
-                                                                  reinterpret_cast<double2 *>(c->obs_xy.p), c->obs_w.p, c->obs_flags.p); LAUNCH_CHECK();
-  c->launches++;
+  if ((rc = launch(c, setup_gather_xy_kernel, (unsigned)((no + 255) / 256), 256, 0, c->d_perm.p, reinterpret_cast<const double2 *>(raw_xy.p), raw_w.p, raw_fl.p, no,
+                   reinterpret_cast<double2 *>(c->obs_xy.p), c->obs_w.p, c->obs_flags.p))) return rc;
   if ((rc = omvg_ba_reset(c))) return rc;
   OMVG_CUDA(cudaStreamSynchronize(s));
   guard.release();
@@ -648,35 +925,16 @@ int omvg_ba_run(omvg_ba_ctx *c, const omvg_ba_options *O, omvg_ba_summary *sum) 
   if (!c || !O || !sum) return fail(OMVG_E_ARG, "null argument");
   OMVG_CUDA(cudaSetDevice(c->device));
   std::memset(sum, 0, sizeof *sum);
-  const Masks m = make_masks(c, O);
-  OMVG_CUDA(cudaMemcpyAsync(c->intr_mask.p, m.intr_mask.data(), c->ni * sizeof(unsigned), cudaMemcpyHostToDevice, c->stream));
+  Plan p; int rc = plan_run(c, O, p); if (rc) return rc;
+  OMVG_CUDA(cudaMemcpyAsync(c->intr_mask.p, p.m.intr_mask.data(), c->ni * sizeof(unsigned), cudaMemcpyHostToDevice, c->stream));
   OMVG_CUDA(cudaMemsetAsync(c->fail.p, 0, sizeof(int), c->stream));
   const long long launches0 = c->launches;
   OMVG_CUDA(cudaEventRecord(c->ev0, c->stream));
-  int rc; bool have_scale = false;
+  bool have_scale = false;
   double jac_ms = 0; long long jac_launches = 0;
   auto account_jac = [&]() { float ms = 0; cudaEventSynchronize(c->evj1); cudaEventElapsedTime(&ms, c->evj0, c->evj1); jac_ms += ms; ++jac_launches; };
 
-  if ((rc = eval_jac(c, O, m, 0, have_scale, true))) return rc;
-  // small reduced systems are solved directly by one CTA (dense_solve_kernel): no gauge / coarse space / PCG
-  const int dense_max = getenv("OMVG_BA_DENSE_MAX") ? std::min(DENSE_MAX, atoi(getenv("OMVG_BA_DENSE_MAX"))) : DENSE_MAX;
-  const bool use_dense1 = 6 * c->nc + c->ni8 <= dense_max;                      // one CTA, shared memory
-  const int dense2_max = getenv("OMVG_BA_DENSE2_MAX") ? std::min(1024, atoi(getenv("OMVG_BA_DENSE2_MAX"))) : 640;
-  const bool use_dense2 = !use_dense1 && 6 * c->nc + c->ni8 <= dense2_max;      // explicit inverse by the blocked Gauss-Jordan kernel
-  const bool use_dense = use_dense1 || use_dense2;
-  int nw = 0;
-  if (!use_dense && (rc = make_gauge(c, m, nw))) return rc;
-  int n_free_intr = 0; for (unsigned mm : m.intr_mask) n_free_intr += __builtin_popcount(mm);
-  // up to 32 free intrinsic columns the block PCG (pcg5 / pcg3) eliminates the intrinsics border; beyond that pcg_kernel
-  // iterates on the whole reduced system.  OMVG_BA_PCG1 forces pcg_kernel, so that tests can cross-check the two.
-  const bool use_block_pcg = n_free_intr <= MAXRHS - 1 && !getenv("OMVG_BA_PCG1");
-  // the per-observation kernels gather pose records (176 B x n_poses) and points through L1: give them all of it
-  OMVG_CUDA(cudaFuncSetAttribute(eval_kernel<true, 4, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 0));
-  OMVG_CUDA(cudaFuncSetAttribute(eval_kernel<false, 8, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 0));
-  OMVG_CUDA(cudaFuncSetAttribute(eval_kernel<true, 4, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 0));
-  OMVG_CUDA(cudaFuncSetAttribute(eval_kernel<false, 8, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 0));
-  OMVG_CUDA(cudaFuncSetAttribute(pcg3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(Pcg2Smem) + 4 * PCG3_NCO_MAX * sizeof(double))));
-  if ((rc = read_scalars(c))) return rc;
+  if ((rc = eval_jac(c, O, p.m, 0, have_scale)) || (rc = make_gauge(c, p)) || (rc = read_scalars(c))) return rc;
   account_jac();
   double x_cost = c->h_scal[S_COST];
   double gmax = host_gmax(c);
@@ -687,17 +945,7 @@ int omvg_ba_run(omvg_ba_ctx *c, const omvg_ba_options *O, omvg_ba_summary *sum) 
   bool step_is_successful = true, failure = false;
   double reference_cost = x_cost, accumulated_reference = 0.0, current_cost = x_cost;
   long long pcg_total = 0;
-  int coarse_age = -1; double last_pcg_its = 0, fresh_pcg_its = 1e30; bool fresh_pending = false;
-  static const int coarse_every = getenv("OMVG_BA_COARSE_EVERY") ? std::max(1, atoi(getenv("OMVG_BA_COARSE_EVERY"))) : 3;
-  // Small reduced systems are latency-bound on the grid-wide barriers of the PCG (4-5 us per iteration of pure
-  // synchronisation at 148 CTAs): up to `small_nc` poses ONE CTA runs the whole solve with block barriers instead.
-  // (measured: 0.70 vs 0.74 ms per LM iteration at 10 poses, but 0.99 vs 0.84 at 20: one CTA serialises the SpMV)
-  static const int small_nc = getenv("OMVG_BA_PCG_SMALL") ? atoi(getenv("OMVG_BA_PCG_SMALL")) : 12;
-  const int pcg_grid = (c->nc <= small_nc && use_block_pcg) ? 1 : c->n_sms;
-  if (!c->gj_grid) {                                        // as many co-resident CTAs as the tile count can use
-    int per_sm = 1; OMVG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, coarse_invert_kernel, 256, 0));
-    c->gj_grid = c->n_sms * std::max(1, std::min(per_sm, 2));
-  }
+  CoarseState coarse;
 
   for (;;) {
     if (step_is_successful) ++n_success; else ++n_fail;
@@ -705,181 +953,12 @@ int omvg_ba_run(omvg_ba_ctx *c, const omvg_ba_options *O, omvg_ba_summary *sum) 
     if (step_is_successful && gmax <= O->gradient_tolerance) { termination = 2; break; }
     if (radius <= O->min_radius) { termination = 4; break; }
     ++iteration;
-    // ---- LM diagonal (levenberg_marquardt_strategy.cc:75-87); diag_* always belong to the current J
-    { Diag3 DG{}; DG.s[0] = Diag3Seg{c->diag_pt.p, c->lmD_pt.p, 3 * c->np}; DG.s[1] = Diag3Seg{c->diag_cam.p, c->lmD_cam.p, 6 * c->nc}; DG.s[2] = Diag3Seg{c->diag_intr.p, c->lmD_intr.p, c->ni8};
-      const int nb = std::max(1, std::min(2 * c->n_sms, (3 * c->np + 255) / 256));
-      lm_diag3_kernel<<<dim3(nb, 3), 256, 0, c->stream>>>(DG, O->min_lm_diagonal, O->max_lm_diagonal, radius); LAUNCH_CHECK(); }
-    // ---- reduced camera system.  schur_stage writes H and the landmarks' {v, G}; schur_gather stores the camera blocks,
-    // schur_border the intrinsics border and the camera right-hand side, corner / corner_final the intrinsics corner and its
-    // right-hand side, all without atomics; then schur_kernel adds the landmarks outside the co-visibility lists (n_slow)
-    // with atomics.  With constant structure the reduced system is its radius-independent part: Scc = diag(Fc'Fc) (stored
-    // by schur_border), Sci = Fi'Fc, Sii = Fi'Fi.
-    { Zero4 Z{}; Z.p[0] = c->Scc.p; Z.n[0] = m.pts_free ? 0 : (long long)c->nnzb * 36;
-      Z.p[1] = c->Sci.p; Z.n[1] = c->n_slow > 0 ? (long long)c->Sci.n : 0; Z.p[2] = c->Sii.p; Z.n[2] = c->n_slow > 0 ? (long long)c->Sii.n : 0;
-      if (Z.n[0] || Z.n[1]) {
-        const int nb = (int)std::max<long long>(1, std::min<long long>(4 * c->n_sms, (std::max(Z.n[0], Z.n[1]) + 255) / 256));
-        zero4_kernel<<<dim3(nb, 3), 256, 0, c->stream>>>(Z); LAUNCH_CHECK(); c->launches++;
-      } }
-    SchurArgs SA{}; SA.Jp = c->Jp.p; SA.Jc = c->Jc.p; SA.Ji = c->Ji.p; SA.EtE = c->EtE.p; SA.Etb = c->Etb.p; SA.EtFi = c->EtFi.p; SA.lmD_pt = c->lmD_pt.p; SA.pt_single = c->pt_single.p;
-    SA.obs_pose = c->obs_pose.p; SA.obs_intr = c->obs_intr.p; SA.obs_pt = c->obs_pt.p; SA.pt_start = c->pt_start.p; SA.n = c->no; SA.n_poses = c->nc; SA.n_intr = c->ni;
-    SA.kiu = c->kiu; SA.bsr = Bsr{c->bitmap.p, c->wprefix.p, c->rowptr.p, c->words}; SA.Scc = c->Scc.p; SA.Sci = c->Sci.p; SA.Sii = c->Sii.p; SA.rhs = c->rhs.p;
-    SA.Einv = c->Einv.p; SA.fail = c->fail.p;
-    const BorderArgs BA{m.pts_free ? c->H.p : nullptr, c->Gv.p, c->FiFc.p, c->g_cam.p, c->FtF.p, c->cam_seg.p, c->seg_start.p, c->seg_intr.p, c->cam_obs.p, c->obs_pt.p,
-                        c->nc, c->Sci.p, c->rhs.p, m.pts_free ? nullptr : c->Scc.p, SA.bsr};
-    const unsigned sg = (unsigned)((c->no + SCHUR_THREADS - 1) / SCHUR_THREADS);
-    const dim3 cg(c->corner_chunks, c->ni);
-    // (kernels instantiated for the intrinsic columns in use, as the column sums are)
-#define STAGE(K) schur_stage_kernel<K><<<sg, SCHUR_THREADS, 0, c->stream>>>(SA, c->H.p, c->Gv.p)
-#define BORDER(K) schur_border_kernel<K><<<c->nc, CCS_THREADS, 0, c->stream>>>(BA)
-#define CORNER(K) corner_kernel<K><<<cg, CORNER_THREADS, 0, c->stream>>>(c->Gv.p, c->pt_start.p, c->pt_single.p, c->obs_intr.p, c->np, c->corner_chunks, c->corner_part.p)
-#define KIU_SWITCH(L) switch (c->kiu) { case 3: L(3); break; case 4: L(4); break; case 6: L(6); break; case 7: L(7); break; default: L(8); break; }
-    if (m.pts_free) {
-      KIU_SWITCH(STAGE); LAUNCH_CHECK();
-      GatherArgs G{c->H.p, c->FtF.p, c->pair.p, c->pair_start.p, c->chunk_blk.p, c->chunk_first.p, c->brow.p, c->cols.p, SA.bsr, c->Scc.p, c->gpart.p, c->ticket.p, c->n_chunks};
-      schur_gather_kernel<<<(c->n_chunks + 7) / 8, 256, 0, c->stream>>>(G); LAUNCH_CHECK();
-      KIU_SWITCH(CORNER); LAUNCH_CHECK();
-      c->launches += 3;
-    }
-    KIU_SWITCH(BORDER); LAUNCH_CHECK();
-    corner_final_kernel<<<c->ni * 72, 128, 0, c->stream>>>(m.pts_free ? c->corner_part.p : nullptr, c->corner_chunks, c->nc, c->ni, c->FiFi.p, c->g_intr.p, c->Sii.p, c->rhs.p); LAUNCH_CHECK();
-    c->launches += 2;
-#undef STAGE
-#undef BORDER
-#undef CORNER
-#undef KIU_SWITCH
-    if (m.pts_free && c->n_slow > 0) {
-      schur_kernel<<<sg, SCHUR_THREADS, 0, c->stream>>>(SA); LAUNCH_CHECK();
-      mirror_kernel<<<(c->nc * 32 + 255) / 256, 256, 0, c->stream>>>(c->Scc.p, SA.bsr, c->cols.p, c->nc); LAUNCH_CHECK(); c->launches += 2;
-    }
-    finish_cam_kernel<<<(c->nc + 63) / 64, 64, 0, c->stream>>>(c->Scc.p, SA.bsr, c->lmD_cam.p, m.pose_mask, c->nc, c->Minv_c.p, c->fail.p, use_dense ? 0 : 1); LAUNCH_CHECK();
-    finish_intr_kernel<<<1, 256, 0, c->stream>>>(c->Sii.p, c->lmD_intr.p, c->intr_mask.p, c->ni8, c->Minv_i.p, c->work_i.p, c->fail.p, (use_block_pcg || use_dense) ? 0 : 1); LAUNCH_CHECK();
-    // ---- PCG on S z = rhs
-    PcgArgs PA{}; PA.Scc = c->Scc.p; PA.rowptr = c->rowptr.p; PA.cols = c->cols.p; PA.Sci = c->Sci.p; PA.Sii = c->Sii.p; PA.rhs = c->rhs.p; PA.Minv_c = c->Minv_c.p; PA.Minv_i = c->Minv_i.p;
-    PA.n_poses = c->nc; PA.ni8 = c->ni8; PA.z = c->z.p; PA.res = c->res.p; PA.p = c->pvec.p; PA.w = c->w.p; PA.zeta = c->zeta.p; PA.part = c->pcg_part.p;
-    PA.tol = O->pcg_tolerance; PA.max_iter = O->pcg_max_iterations; PA.out = c->scal.p + S_PCG_IT;
-    // ---- coarse operator of the two-level preconditioner (aggregated gauge space), shared by all PCG kernels.
-    // It is only a preconditioner: a slightly stale E^-1 (previous LM step, radius/3) costs a few extra PCG
-    // iterations (measured 38->40, 42->49, 43->43) but saves its O(nco^3) setup, so it is refreshed every
-    // `coarse_every` LM steps (measured at 1000 cameras, ms per solve: every step 17.9, 2: 16.0, 3: 15.2, 5: 15.9),
-    // or earlier if the last solve needed 1.5x the iterations seen right after a refresh.
-    // Without one (a single pose, or no gauge freedom) the PCG is block-Jacobi alone: nw = nco = 0, as pcg3 reads both.
-    const bool use_coarse = !use_dense && nw > 0 && c->nc >= 2;
-    const Coarse CO{c->agg_of.p, c->agg_start.p, c->agg_cams.p, c->ng, use_coarse ? nw : 0, use_coarse ? c->ng * nw : 0};
-    if (use_coarse) {
-      const int nco = CO.nco;
-      const bool refresh = nco > 0 && (coarse_age < 0 || coarse_age >= coarse_every || last_pcg_its > 1.5 * fresh_pcg_its + 5);
-      if (refresh) { coarse_age = 0; fresh_pending = true; }
-      ++coarse_age;
-      if (refresh) {
-        OMVG_CUDA(cudaMemsetAsync(c->cE.p, 0, (size_t)nco * nco * sizeof(double), c->stream));
-        coarse_assemble_kernel<<<(c->nnzb + 127) / 128, 128, 0, c->stream>>>(c->Scc.p, c->brow.p, c->cols.p, c->nnzb, c->gW.p, c->nc, CO, c->cE.p); LAUNCH_CHECK();
-        // blocked Gauss-Jordan, in place: cE becomes E^-1
-        double *Ep = c->cE.p, *Tp = c->cT.p; int nn = nco; int *fp = c->fail.p;
-        static const bool gj_timing = getenv("OMVG_BA_GJ_TIMING") != nullptr;
-        unsigned long long *tp = nullptr;
-        if (gj_timing) { if (!c->pcg_tim.p) { if ((rc = c->pcg_tim.alloc(8))) return rc; } OMVG_CUDA(cudaMemsetAsync(c->pcg_tim.p, 0, 64, c->stream)); tp = c->pcg_tim.p; }
-        void *cargs[] = {&Ep, &nn, &Tp, &fp, &tp};
-        const int mt = (nco + CT - 1) / CT;                     // no more CTAs than 64x64 tiles: a small coarse space pays for fewer barrier participants
-        const int gj = std::max(1, std::min(c->gj_grid, mt * mt));
-        OMVG_CUDA(cudaLaunchCooperativeKernel((void *)coarse_invert_kernel, dim3(gj), dim3(256), cargs, 0, c->stream));
-        if (gj_timing) { unsigned long long h[8]; OMVG_CUDA(cudaMemcpyAsync(h, c->pcg_tim.p, 64, cudaMemcpyDeviceToHost, c->stream)); OMVG_CUDA(cudaStreamSynchronize(c->stream));
-          fprintf(stderr, "[omvg_ba gj timing] us: pivot inverse %.1f slices %.1f sync %.1f tiles %.1f sync %.1f (n %d, %d CTAs)\n", h[0] * 1e-3, h[1] * 1e-3, h[2] * 1e-3, h[3] * 1e-3, h[4] * 1e-3, nco, c->gj_grid); }
-        c->launches += 2;
-      }
-    }
-    if (use_dense2) {
-      int nd = 6 * c->nc + c->ni8;
-      if (!c->dA.p) { if ((rc = c->dA.alloc((size_t)nd * nd)) || (rc = c->dT.alloc(3 * (size_t)GJ_B * nd))) return rc; }
-      OMVG_CUDA(cudaMemsetAsync(c->dA.p, 0, (size_t)nd * nd * sizeof(double), c->stream));
-      dense_assemble_kernel<<<std::max(1, std::min(4 * c->n_sms, (36 * c->nnzb + 255) / 256)), 256, 0, c->stream>>>(c->Scc.p, c->brow.p, c->cols.p, c->nnzb, c->Sci.p, c->Sii.p, c->nc, c->ni8, c->dA.p); LAUNCH_CHECK();
-      double *Ap = c->dA.p, *Tp = c->dT.p; int *fp = c->fail.p; unsigned long long *tp = nullptr;
-      void *cargs[] = {&Ap, &nd, &Tp, &fp, &tp};
-      const int mt = (nd + CT - 1) / CT;
-      OMVG_CUDA(cudaLaunchCooperativeKernel((void *)coarse_invert_kernel, dim3(std::max(1, std::min(c->gj_grid, mt * mt))), dim3(256), cargs, 0, c->stream));
-      dense_apply_kernel<<<(nd * 32 + 255) / 256, 256, 0, c->stream>>>(c->dA.p, c->rhs.p, nd, c->z.p, c->scal.p + S_PCG_IT); LAUNCH_CHECK();
-      c->launches += 3;
-    } else
-    if (use_dense1) {
-      const int nd = 6 * c->nc + c->ni8;
-      const size_t dsm = ((size_t)nd * (nd + 1) / 2 + (3 + DENSE_NB) * (size_t)nd) * sizeof(double);
-      // The attribute is process-wide: set it to what any system size may need, never to this call's dsm, so that a
-      // smaller solve on another host thread cannot lower it under this launch.
-      static const int dense_smem_max = [] { int v = 0, dev = 0; cudaFuncAttributes fa{}; cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev); cudaFuncGetAttributes(&fa, dense_solve_kernel); return v - (int)fa.sharedSizeBytes; }();
-      OMVG_CUDA(cudaFuncSetAttribute(dense_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dense_smem_max));
-      static const bool dense_timing = getenv("OMVG_BA_DENSE_TIMING") != nullptr;
-      unsigned long long *tp = nullptr;
-      if (dense_timing) { if (!c->pcg_tim.p) { if ((rc = c->pcg_tim.alloc(8))) return rc; } OMVG_CUDA(cudaMemsetAsync(c->pcg_tim.p, 0, 64, c->stream)); tp = c->pcg_tim.p; }
-      dense_solve_kernel<<<1, 1024, dsm, c->stream>>>(c->Scc.p, c->rowptr.p, c->cols.p, c->Sci.p, c->Sii.p, c->rhs.p, c->nc, c->ni8, c->z.p, c->fail.p, c->scal.p + S_PCG_IT, tp); LAUNCH_CHECK();
-      if (dense_timing) { unsigned long long h[8]; OMVG_CUDA(cudaMemcpyAsync(h, c->pcg_tim.p, 64, cudaMemcpyDeviceToHost, c->stream)); OMVG_CUDA(cudaStreamSynchronize(c->stream));
-        fprintf(stderr, "[omvg_ba dense timing] n %d us: assemble %.1f factor %.1f backward %.1f\n", nd, h[0] * 1e-3, h[1] * 1e-3, h[2] * 1e-3); }
-    } else
-    if (use_block_pcg) {
-      Pcg2Args P2{}; P2.Scc = c->Scc.p; P2.rowptr = c->rowptr.p; P2.cols = c->cols.p; P2.Sci = c->Sci.p; P2.Sii = c->Sii.p; P2.rhs = c->rhs.p; P2.Minv_c = c->Minv_c.p;
-      P2.W = c->gW.p; P2.intr_mask = c->intr_mask.p; P2.n_poses = c->nc; P2.ni8 = c->ni8; P2.X = c->bX.p; P2.Rv = c->bR.p; P2.Pv = c->bP.p; P2.Wv = c->bW.p; P2.Zv = c->bZ.p;
-      P2.part = c->pcg2_part.p; P2.z = c->z.p; P2.tol = O->pcg_tolerance; P2.max_iter = O->pcg_max_iterations; P2.out = c->scal.p + S_PCG_IT;
-      Pcg3Args P3{}; P3.base = P2; P3.C = CO; P3.Einv = c->cE.p; P3.Cv = c->cCv.p; P3.Yv = c->cYv.p; P3.Pv2 = c->bP2.p;
-      static const bool pcg_timing = getenv("OMVG_BA_PCG_TIMING") != nullptr;
-      if (pcg_timing) { if (!c->pcg_tim.p) { if ((rc = c->pcg_tim.alloc(8))) return rc; } OMVG_CUDA(cudaMemsetAsync(c->pcg_tim.p, 0, 64, c->stream)); P3.tim = c->pcg_tim.p; }
-      // pcg5: shared-memory resident, aggregate-owned (2 barriers + 2 L2 round trips per iteration).  Needs one CTA per
-      // aggregate, <= 4 right-hand sides (1 + free intrinsic columns) and aggregates of <= PCG5_MC cameras; else pcg3,
-      // on one CTA up to small_nc poses.
-      const int nrhs_host = 1 + n_free_intr;
-      if (pcg_grid > 1 && nrhs_host <= PCG5_NR && c->ng <= pcg_grid && c->agg_maxsize <= PCG5_MC && c->nb_max <= PCG5_NB && P3.C.nco <= PCG3_NCO_MAX) {
-        const size_t fixed = sizeof(Pcg5Red) + sizeof(Pcg5Smem) + (size_t)PCG5_NR * PCG3_NCO_MAX * sizeof(double) + (size_t)PCG5_NB * PCG5_PS * sizeof(double);
-        static const int smem_max = [] { int v = 0, dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev); return v; }();
-        const int nb_cache = (int)std::max<long long>(0, ((long long)smem_max - (long long)fixed - 2048) /   /* (static shared memory of the kernel + slack) */ (long long)(PCG5_BS * sizeof(double) + sizeof(unsigned short)));
-        const size_t smem = fixed + (size_t)nb_cache * (PCG5_BS * sizeof(double) + sizeof(unsigned short)) + 16;
-        OMVG_CUDA(cudaFuncSetAttribute(pcg5_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        double *cg2 = c->cCv2.p, *aw = c->cAW.p; int nbc = nb_cache; const int *nbs = c->nb_start.p, *nbl = c->nb_list.p; const unsigned short *lc = c->blk_lcol.p;
-        void *args[] = {&P3, &cg2, &aw, &nbc, &nbs, &nbl, &lc};
-        // one CTA per aggregate and no more: idle CTAs would only add participants to the two barriers of every iteration
-        OMVG_CUDA(cudaLaunchCooperativeKernel((void *)pcg5_kernel, dim3(std::max(1, c->ng)), dim3(PCG2_THREADS), args, smem, c->stream));
-        if (pcg_timing) { unsigned long long h[8]; OMVG_CUDA(cudaMemcpyAsync(h, c->pcg_tim.p, 64, cudaMemcpyDeviceToHost, c->stream)); OMVG_CUDA(cudaStreamSynchronize(c->stream));
-          fprintf(stderr, "[omvg_ba pcg5 timing] us: A wait-AW %.1f y %.1f local %.1f reduce %.1f | B gather %.1f rows %.1f publish %.1f reduce %.1f (cache %d blocks)\n", h[0] * 1e-3, h[1] * 1e-3, h[2] * 1e-3, h[3] * 1e-3, h[6] * 1e-3, h[7] * 1e-3, h[4] * 1e-3, h[5] * 1e-3, nb_cache); }
-      } else {
-        void *args[] = {&P3};
-        OMVG_CUDA(cudaLaunchCooperativeKernel((void *)pcg3_kernel, dim3(pcg_grid), dim3(PCG2_THREADS), args, sizeof(Pcg2Smem) + 4 * PCG3_NCO_MAX * sizeof(double), c->stream));
-        if (pcg_timing) { unsigned long long h[8]; OMVG_CUDA(cudaMemcpyAsync(h, c->pcg_tim.p, 64, cudaMemcpyDeviceToHost, c->stream)); OMVG_CUDA(cudaStreamSynchronize(c->stream));
-          fprintf(stderr, "[omvg_ba pcg timing] us: coarse (stage %.1f rows %.1f sync %.1f) z %.1f spmv %.1f update %.1f tail %.1f border %.1f\n", h[6] * 1e-3, h[7] * 1e-3, h[0] * 1e-3, h[1] * 1e-3, h[2] * 1e-3, h[3] * 1e-3, h[4] * 1e-3, h[5] * 1e-3); }
-      }
-    } else {
-      // more than 32 free intrinsic columns (e.g. one intrinsic group per image): PCG on the whole reduced system
-      // [Scc Sci'; Sci Sii] with the same aggregated coarse space on the camera rows and block-Jacobi on the intrinsics
-      if (use_coarse) { PA.W = c->gW.p; PA.C = CO; PA.Einv = c->cE.p; PA.Cv = c->cCv.p; PA.Yv = c->cYv.p; }
-      void *args[] = {&PA}; OMVG_CUDA(cudaLaunchCooperativeKernel((void *)pcg_kernel, dim3(pcg_grid), dim3(256), args, 0, c->stream));
-    }
-    // ---- back substitution, step = -y (constant structure: the landmark step stays zero)
-    OMVG_CUDA(cudaMemsetAsync(c->step_pt.p, 0, 3 * (size_t)c->np * sizeof(double), c->stream));
-    if (m.pts_free) {
-      backsub_obs_kernel<<<(unsigned)((c->no + 255) / 256), 256, 0, c->stream>>>(c->Jp.p, c->Jc.p, c->Ji.p, c->obs_pose.p, c->obs_intr.p, c->obs_pt.p, c->nc, c->no, c->kiu, c->z.p, c->step_pt.p); LAUNCH_CHECK();
-      backsub_point_kernel<<<(c->np + 255) / 256, 256, 0, c->stream>>>(c->Etb.p, c->Einv.p, c->pt_start.p, c->np, m.pts_free, c->step_pt.p); LAUNCH_CHECK();
-      c->launches += 2;
-    }
-    negate_kernel<<<(c->nred + 255) / 256, 256, 0, c->stream>>>(c->z.p, c->nred, c->step_red.p); LAUNCH_CHECK();
-    // ---- model cost change
-    model_kernel<<<c->eval_blocks, MODEL_THREADS, 0, c->stream>>>(c->r.p, c->Jp.p, c->Jc.p, c->Ji.p, c->obs_pose.p, c->obs_intr.p, c->obs_pt.p, c->no, c->nc, c->kiu, c->step_pt.p, c->step_red.p, c->part.p); LAUNCH_CHECK();
-    c->launches += 6;
-    if (c->npri) { prior_model_kernel<<<1, PRIOR_THREADS, 0, c->stream>>>(c->JP.p, c->rP.p, c->prior_pose.p, c->npri, c->step_red.p, c->part.p + c->eval_blocks); LAUNCH_CHECK(); c->launches++; }
-    if ((rc = reduce_to(c, c->part.p, c->eval_blocks + (c->npri ? 1 : 0), S_MODEL))) return rc;
-    // ---- candidate = Plus(x, step * scale)
-    const int ub = 64;
-    auto update_all = [&]() -> int {       // candidate = Plus(x, step * scale) for the three parameter blocks; |step|^2 and |x|^2 into S_STEP2_* / S_X2_*
-      Upd3 U{};
-      U.s[0] = UpdSeg{c->pt[0].p, c->step_pt.p, c->sc_pt.p, 3 * c->np, 3, m.pts_free ? 7u : 0u, m.pts_free ? c->pt_mask.p : nullptr, c->pt[1].p};
-      U.s[1] = UpdSeg{c->pose[0].p, c->step_red.p, c->sc_cam.p, 6 * c->nc, 6, m.pose_mask, nullptr, c->pose[1].p};
-      U.s[2] = UpdSeg{c->intr[0].p, c->step_red.p + 6 * c->nc, c->sc_intr.p, c->ni8, KI, 0u, c->intr_mask.p, c->intr[1].p};
-      update3_kernel<<<dim3(ub, 3), 256, 0, c->stream>>>(U, c->part3.p); LAUNCH_CHECK();
-      static_assert(S_STEP2_POSE == S_STEP2_PT + 1 && S_STEP2_INTR == S_STEP2_PT + 2 && S_X2_PT == S_STEP2_PT + 3 && S_X2_POSE == S_STEP2_PT + 4 && S_X2_INTR == S_STEP2_PT + 5, "slot order");
-      reduce_multi_kernel<<<6, 1024, 0, c->stream>>>(c->part3.p, ub, c->scal.p + S_STEP2_PT); LAUNCH_CHECK();
-      c->launches += 2; return OMVG_OK;
-    };
-    if ((rc = update_all())) return rc;
-    if ((rc = eval_cost(c, O, 1, S_CAND_COST))) return rc;
-    if ((rc = read_scalars(c))) return rc;
+    // ---- the LM step (levenberg_marquardt_strategy.cc:65-160) by the Schur complement, candidate = Plus(x, step) and its cost
+    if ((rc = lm_diagonal(c, O, radius)) || (rc = assemble_reduced(c, p)) || (rc = refresh_coarse(c, p, coarse)) || (rc = solve_reduced(c, O, p)) ||
+        (rc = back_substitute(c, p)) || (rc = update_all(c, p.m)) || (rc = eval_cost(c, O, 1, S_CAND_COST)) || (rc = read_scalars(c))) return rc;
     const double *h = c->h_scal;
     pcg_total += (long long)h[S_PCG_IT];
-    last_pcg_its = h[S_PCG_IT]; if (fresh_pending) { fresh_pcg_its = last_pcg_its; fresh_pending = false; }
+    coarse.solved(h[S_PCG_IT]);
     int failflag; std::memcpy(&failflag, c->h_scal + S_COUNT + 192, sizeof(int));
     const double model_cost_change = h[S_MODEL];
     bool finite_step = std::isfinite(h[S_STEP2_PT]) && std::isfinite(h[S_STEP2_POSE]) && std::isfinite(h[S_STEP2_INTR]) && std::isfinite(model_cost_change);
@@ -902,12 +981,9 @@ int omvg_ba_run(omvg_ba_ctx *c, const omvg_ba_options *O, omvg_ba_summary *sum) 
     const double rho = std::max(rel, hist);
     if (rho > O->min_relative_decrease) {                    // HandleSuccessfulStep (:767-780)
       std::swap(c->pose[0].p, c->pose[1].p); std::swap(c->intr[0].p, c->intr[1].p); std::swap(c->pt[0].p, c->pt[1].p); std::swap(c->camR[0].p, c->camR[1].p); std::swap(c->camrec[0].p, c->camrec[1].p);
-      // |x| of the accepted iterate = sqrt(|x_old|^2 ...) is not reusable: recompute from the candidate norms
-      if ((rc = eval_jac(c, O, m, 0, have_scale, true))) return rc;
-      if (!use_dense && (rc = make_gauge(c, m, nw))) return rc;
-      // x_norm of the new x: update3_kernel measures |x| of its input: one more pass over the new x
-      if ((rc = update_all())) return rc;     // (the gradient maxima of eval_jac sit in part2, the norm partials in part3)
-      if ((rc = read_scalars(c))) return rc;
+      // |x| of the accepted iterate = sqrt(|x_old|^2 ...) is not reusable: update3_kernel measures |x| of its input, so
+      // one more pass over the new x gives it (the gradient maxima of eval_jac sit in part2, the norm partials in part3)
+      if ((rc = eval_jac(c, O, p.m, 0, have_scale)) || (rc = make_gauge(c, p)) || (rc = update_all(c, p.m)) || (rc = read_scalars(c))) return rc;
       account_jac();
       x_cost = c->h_scal[S_COST]; gmax = host_gmax(c);
       x_norm = std::sqrt(c->h_scal[S_X2_PT] + c->h_scal[S_X2_POSE] + c->h_scal[S_X2_INTR]);
@@ -1000,14 +1076,8 @@ static int ensure_perm(omvg_ba_ctx *c) {
 int omvg_ba_residual_norms(omvg_ba_ctx *c, double *norms) {
   if (!c || !norms) return fail(OMVG_E_ARG, "null argument");
   OMVG_CUDA(cudaSetDevice(c->device));
-  { const int prc = ensure_perm(c); if (prc) return prc; }
-  omvg_ba_options O; omvg_ba_default_options(&O); O.use_loss = 0;
-  cam_prep_kernel<<<(c->nc + 127) / 128, 128, 0, c->stream>>>(c->pose[0].p, c->nc, c->camR[0].p, c->camdR.p, c->camrec[0].p); LAUNCH_CHECK();
-  EvalArgs A{}; A.poses = c->pose[0].p; A.intr = c->intr[0].p; A.pts = c->pt[0].p; A.camR = c->camR[0].p; A.camdR = c->camdR.p; A.camrec = c->camrec[0].p;
-  A.obs_xy = c->obs_xy.p; A.intr_model = c->intr_model.p; A.obs_pose = c->obs_pose.p; A.obs_intr = c->obs_intr.p; A.obs_pt = c->obs_pt.p;
-  A.n_obs = c->no; A.use_loss = 0; A.huber_a = O.huber_a; A.cost_partial = c->part.p; A.rnorm = c->r.p;   // r is scratch between solves
-  eval_kernel<false, 8, false><<<c->eval_grid, EVAL_THREADS, 0, c->stream>>>(A); LAUNCH_CHECK();   // (weights deliberately not applied: pixels)
-  c->launches += 2;
+  int rc = ensure_perm(c); if (rc) return rc;
+  if ((rc = eval_pixel_norms(c))) return rc;
   std::vector<double> h(c->no);
   OMVG_CUDA(cudaMemcpyAsync(h.data(), c->r.p, (size_t)c->no * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   OMVG_CUDA(cudaStreamSynchronize(c->stream));
@@ -1043,9 +1113,9 @@ static int ensure_reject_state(omvg_ba_ctx *c) {
   if (c->pt_fixed.p) OMVG_CUDA(cudaMemcpyAsync(c->pt_gcp.p, c->pt_fixed.p, c->np, cudaMemcpyDeviceToDevice, c->stream));   // fixed at create = control points
   else OMVG_CUDA(cudaMemsetAsync(c->pt_gcp.p, 0, c->np, c->stream));
   OMVG_CUDA(cudaMemsetAsync(c->pt_removed.p, 0, c->np, c->stream));
-  if (!c->obs_w.p) { if ((rc = c->obs_w.alloc(c->no))) return rc; fill_kernel<<<gb, 256, 0, c->stream>>>(c->obs_w.p, c->no, 1.0); LAUNCH_CHECK(); c->launches++; }
+  if (!c->obs_w.p && ((rc = c->obs_w.alloc(c->no)) || (rc = launch(c, fill_kernel, gb, 256, 0, c->obs_w.p, c->no, 1.0)))) return rc;
   if (!c->pt_fixed.p) { if ((rc = c->pt_fixed.alloc(c->np))) return rc; OMVG_CUDA(cudaMemsetAsync(c->pt_fixed.p, 0, c->np, c->stream)); }
-  if (!c->pt_mask.p) { if ((rc = c->pt_mask.alloc(c->np))) return rc; fill_u32_kernel<<<gp, 256, 0, c->stream>>>(c->pt_mask.p, c->np, 7u); LAUNCH_CHECK(); c->launches++; }
+  if (!c->pt_mask.p && ((rc = c->pt_mask.alloc(c->np)) || (rc = launch(c, fill_u32_kernel, gp, 256, 0, c->pt_mask.p, c->np, 7u)))) return rc;
   c->has_ext = true; c->reject_ready = true;
   return OMVG_OK;
 }
@@ -1069,16 +1139,10 @@ int omvg_ba_reject_outliers(omvg_ba_ctx *c, double threshold_px, int32_t min_tra
   int rc = ensure_reject_state(c); if (rc) return rc;
   OMVG_CUDA(cudaMemsetAsync(c->rej_bits.p, 0, c->rej_bits.n * 4, c->stream));
   OMVG_CUDA(cudaMemsetAsync(c->rej_cnt.p, 0, 16, c->stream));
-  // |r| in pixels at the current parameters (no weight, no loss): r is scratch between solves
-  cam_prep_kernel<<<(c->nc + 127) / 128, 128, 0, c->stream>>>(c->pose[0].p, c->nc, c->camR[0].p, c->camdR.p, c->camrec[0].p); LAUNCH_CHECK();
-  EvalArgs A{}; A.poses = c->pose[0].p; A.intr = c->intr[0].p; A.pts = c->pt[0].p; A.camR = c->camR[0].p; A.camdR = c->camdR.p; A.camrec = c->camrec[0].p;
-  A.obs_xy = c->obs_xy.p; A.intr_model = c->intr_model.p; A.obs_pose = c->obs_pose.p; A.obs_intr = c->obs_intr.p; A.obs_pt = c->obs_pt.p;
-  A.n_obs = c->no; A.use_loss = 0; A.huber_a = 16.0; A.cost_partial = c->part.p; A.rnorm = c->r.p;
-  eval_kernel<false, 8, false><<<c->eval_grid, EVAL_THREADS, 0, c->stream>>>(A); LAUNCH_CHECK();
-  reject_obs_kernel<<<(unsigned)((c->no + 255) / 256), 256, 0, c->stream>>>(c->r.p, c->obs_w.p, c->obs_pt.p, c->pt_gcp.p, c->no, threshold_px, c->d_perm.p, c->rej_bits.p, c->rej_cnt.p); LAUNCH_CHECK();
-  reject_tracks_kernel<<<(c->np + 127) / 128, 128, 0, c->stream>>>(c->pt_start.p, c->np, c->obs_w.p, min_track_length, nullptr, c->pt_gcp.p, c->d_perm.p, c->rej_bits.p,
-                                                                 c->pt_fixed.p, c->pt_mask.p, c->pt_removed.p, c->pt_now.p, c->rej_cnt.p); LAUNCH_CHECK();
-  c->launches += 4;
+  if ((rc = eval_pixel_norms(c)) ||
+      (rc = launch(c, reject_obs_kernel, (unsigned)((c->no + 255) / 256), 256, 0, c->r.p, c->obs_w.p, c->obs_pt.p, c->pt_gcp.p, c->no, threshold_px, c->d_perm.p, c->rej_bits.p, c->rej_cnt.p)) ||
+      (rc = launch(c, reject_tracks_kernel, (c->np + 127) / 128, 128, 0, c->pt_start.p, c->np, c->obs_w.p, min_track_length, nullptr, c->pt_gcp.p, c->d_perm.p, c->rej_bits.p,
+                   c->pt_fixed.p, c->pt_mask.p, c->pt_removed.p, c->pt_now.p, c->rej_cnt.p))) return rc;
   return reject_finish(c, obs_removed_bits, point_removed, n_outliers, n_tracks);
 }
 
@@ -1090,9 +1154,8 @@ int omvg_ba_remove_points(omvg_ba_ctx *c, const uint8_t *point_mask, uint32_t *o
   OMVG_CUDA(cudaMemcpyAsync(kill.p, point_mask, c->np, cudaMemcpyHostToDevice, c->stream));
   OMVG_CUDA(cudaMemsetAsync(c->rej_bits.p, 0, c->rej_bits.n * 4, c->stream));
   OMVG_CUDA(cudaMemsetAsync(c->rej_cnt.p, 0, 16, c->stream));
-  reject_tracks_kernel<<<(c->np + 127) / 128, 128, 0, c->stream>>>(c->pt_start.p, c->np, c->obs_w.p, 0, kill.p, c->pt_gcp.p, c->d_perm.p, c->rej_bits.p,
-                                                                 c->pt_fixed.p, c->pt_mask.p, c->pt_removed.p, c->pt_now.p, c->rej_cnt.p); LAUNCH_CHECK();
-  c->launches++;
+  if ((rc = launch(c, reject_tracks_kernel, (c->np + 127) / 128, 128, 0, c->pt_start.p, c->np, c->obs_w.p, 0, kill.p, c->pt_gcp.p, c->d_perm.p, c->rej_bits.p,
+                   c->pt_fixed.p, c->pt_mask.p, c->pt_removed.p, c->pt_now.p, c->rej_cnt.p))) return rc;
   return reject_finish(c, obs_removed_bits, nullptr, nullptr, n_tracks);      // (synchronises: `kill` may be released)
 }
 
@@ -1115,15 +1178,11 @@ int omvg_ba_debug_eval(omvg_ba_ctx *c, const omvg_ba_options *O, double *cost, d
   OMVG_CUDA(cudaMemcpyAsync(c->intr_mask.p, m.intr_mask.data(), c->ni * sizeof(unsigned), cudaMemcpyHostToDevice, c->stream));
   // unscaled evaluation (intrinsic columns >= kiu are never written: present them as zeros)
   OMVG_CUDA(cudaMemsetAsync(c->Ji.p, 0, c->Ji.n * sizeof(double), c->stream));
-  cam_prep_kernel<<<(c->nc + 127) / 128, 128, 0, c->stream>>>(c->pose[0].p, c->nc, c->camR[0].p, c->camdR.p, c->camrec[0].p); LAUNCH_CHECK();
-  EvalArgs A{}; A.poses = c->pose[0].p; A.intr = c->intr[0].p; A.pts = c->pt[0].p; A.camR = c->camR[0].p; A.camdR = c->camdR.p; A.camrec = c->camrec[0].p;
-  A.obs_xy = c->obs_xy.p; A.intr_model = c->intr_model.p; A.obs_pose = c->obs_pose.p; A.obs_intr = c->obs_intr.p; A.obs_pt = c->obs_pt.p;
-  A.n_obs = c->no; A.use_loss = O->use_loss; A.huber_a = O->huber_a; A.r = c->r.p; A.Jp = c->Jp.p; A.Jc = c->Jc.p; A.Ji = c->Ji.p;
-  A.cost_partial = c->part.p; A.kiu = c->kiu; A.pose_mask = m.pose_mask; A.intr_mask = c->intr_mask.p; A.pts_free = m.pts_free;
+  EvalArgs A; int rc = eval_prep(c, 0, A); if (rc) return rc;
+  A.use_loss = O->use_loss; A.huber_a = O->huber_a; A.r = c->r.p; A.Jp = c->Jp.p; A.Jc = c->Jc.p; A.Ji = c->Ji.p;
+  A.kiu = c->kiu; A.pose_mask = m.pose_mask; A.intr_mask = c->intr_mask.p; A.pts_free = m.pts_free;
   A.obs_w = c->obs_w.p; A.obs_flags = c->obs_flags.p; A.pt_fixed = c->pt_fixed.p;      // (prior rows are not part of this dump)
-  eval_kernel<true, 4, true><<<c->eval_grid, EVAL_THREADS, 0, c->stream>>>(A); LAUNCH_CHECK();
-  int rc = reduce_to(c, c->part.p, c->eval_grid, S_COST); if (rc) return rc;
-  c->launches += 2;
+  if ((rc = launch(c, eval_kernel<true, 4, true>, c->eval_grid, EVAL_THREADS, 0, A)) || (rc = reduce_to(c, c->part.p, c->eval_grid, S_COST))) return rc;
   const long long n = c->no;
   std::vector<double> hr(2 * n), hp(6 * n), hc(12 * n), hi(2 * KI * n); double hcost = 0;
   OMVG_CUDA(cudaMemcpyAsync(hr.data(), c->r.p, hr.size() * 8, cudaMemcpyDeviceToHost, c->stream));
