@@ -109,6 +109,29 @@ int omvg_match_cascade_prepare(omvg_match_ctx *ctx, const float *primary, const 
  * ascending j; the reference then sorts by (i, j) (IndMatch::getDeduplicated) and drops matches with equal
  * coordinates (IndMatchDecorator) — host-side steps the shim performs with openMVG's own functions. */
 int omvg_match_cascade_run(omvg_match_ctx *ctx, const uint32_t *pair_i, const uint32_t *pair_j, uint64_t n_pairs, float dist_ratio);
+/* ---- guided matching: geometry_aware::GuidedMatching (robust_estimation/guided_matching.hpp:28-68, 178-227), the
+ * "-r" / guided_matching step of ImageCollectionGeometricFilter::Robust_model_estimation (GeometricFilter.hpp:96-123)
+ * for the F, E (as F = K_J^-T E K_I^-1) and H models.  For every feature i of image I, every feature j of image J is
+ * tested with the pair's model and a match is kept as the reference keeps it; same decisions as the reference.
+ * Positions: xy = counts[image] rows of {x, y} in pixels, the positions GuidedMatching uses (get_ud_pixel of the view's
+ * intrinsic when it has one, else the raw feature position).  Device storage is allocated on first use, separate from
+ * the descriptor arena; omvg_match_set_images drops it.  Asynchronous on the context's stream. */
+int omvg_match_upload_positions(omvg_match_ctx *ctx, uint32_t image, const double *xy);
+/* error_model: OMVG_GUIDED_EPIPOLAR = EpipolarDistanceError (F, or F from E), OMVG_GUIDED_TRANSFER = AsymmetricError (H).
+ *   models[n_pairs][9]   row-major 3x3 model of pair p (maps image pair_i[p] to image pair_j[p])
+ *   thresholds[n_pairs]  errorTh: a candidate is in the band iff error < thresholds[p] (GuidedMatching's own argument,
+ *                        i.e. already squared: Square(errorMax) in the filters)
+ *   dist_ratio           GuidedMatching's distRatio (already squared: Square(d_distance_ratio)).  >= 0: the
+ *                        descriptor variant, i kept iff its two smallest L2^2 over the band satisfy bd < dist_ratio * sbd
+ *                        (in double) and matched to the lowest j of distance bd; < 0: the descriptor-free variant, i
+ *                        matched to the lowest j of minimal error.
+ * Needs omvg_match_prepare and positions of every image named.  Fetch with omvg_match_fetch: row p holds (i, j) =
+ * (row in image pair_i[p], row in image pair_j[p]) in ascending i, at most one per i.  OMVG_E_STATE before prepare or for
+ * an image without positions; OMVG_E_ARG for pairs out of range, a non-finite model or threshold, or a NaN dist_ratio. */
+#define OMVG_GUIDED_EPIPOLAR 0
+#define OMVG_GUIDED_TRANSFER 1
+int omvg_match_guided_run(omvg_match_ctx *ctx, int32_t error_model, const uint32_t *pair_i, const uint32_t *pair_j, uint64_t n_pairs,
+                          const double *models, const double *thresholds, double dist_ratio);
 /* Validation aid (tests only): hash codes [count][4] (bit j = bit j&31 of word j>>5), bucket ids [count][6],
  * zero-mean vector [128]; any pointer may be NULL. */
 int omvg_match_cascade_debug_hash(omvg_match_ctx *ctx, uint32_t image, uint32_t *codes, uint16_t *bucket_ids, float *zero_mean);

@@ -24,6 +24,8 @@
 
 #include <cuda.h>
 #include <algorithm>
+#include <cfloat>
+#include <cmath>
 #include <climits>
 #include <cstring>
 #include <vector>
@@ -713,6 +715,124 @@ __global__ void __launch_bounds__(FIN_THREADS) cascade_compact_kernel(const Pair
   if (threadIdx.x == 0) counts[blockIdx.x] = running;
 }
 
+// ================================================================================= guided matching
+// geometry_aware::GuidedMatching (robust_estimation/guided_matching.hpp:28-68 and 178-227) for a list of pairs: every
+// feature i of image I is tested against every feature j of image J with the pair's model, in ascending j.  One block
+// per (pair, 128 features of I), one thread per i; J's positions stream through shared memory in ascending j, so each
+// thread runs the reference's sequential loop for its i and needs no merge.  PairInfo's q_* fields describe I (the
+// side that is iterated) and db_* fields describe J.
+//   error: EpipolarDistanceError (solver_fundamental_kernel.cpp:157-166) or AsymmetricError (solver_homography_kernel.hpp
+//     :59-63).  The per-i sub-expressions (F x and |F x|^2_{0,1}, or the projected point of H x) are hoisted; the
+//     reference evaluates exactly these, so every operation below is the reference's, explicitly rounded (this file
+//     allows FMA contraction).  Built for x86-64-v3, the reference forms each row of M [x; 1] with one FMA, whose
+//     operand order differs between the two errors (DESIGN §3.9); the per-j part and the norms have none.
+//   DESC: distanceRatio<double>::update with the exact integer L2 of the two descriptors (|a|^2 + |b|^2 - 2 a.b, dp4a),
+//     kept iff a second distance exists and bd < ratio * sbd in double.  !DESC: the lowest j of minimal error.
+// out[out_off + i].x = j of the match or -1.
+constexpr int GM_THREADS = 128, GM_CHUNK = 512;
+struct GuidedModel { double M[9]; double thr; };
+
+template <int MODEL, bool DESC>
+__global__ void __launch_bounds__(GM_THREADS)
+guided_match_kernel(const double2 *__restrict__ pos, const uint8_t *__restrict__ desc, const int32_t *__restrict__ norm,
+                    const PairInfo *__restrict__ pairs, const GuidedModel *__restrict__ models, int2 *__restrict__ out,
+                    double ratio) {
+  __shared__ double2 sj[GM_CHUNK];
+  const PairInfo P = pairs[blockIdx.y];
+  if (blockIdx.x * GM_THREADS >= P.q_count) return;               // uniform over the block
+  const uint32_t i = blockIdx.x * GM_THREADS + threadIdx.x;
+  const bool active = i < P.q_count;
+  const double *M = models[blockIdx.y].M;
+  const double thr = models[blockIdx.y].thr;
+  const double2 x = pos[P.q_row0 + (active ? i : 0)];
+  double a0, a1, a2 = 0.0, n = 0.0;
+  if (MODEL == OMVG_GUIDED_EPIPOLAR) {                           // F x: fma(F_k1, y, F_k0 x) + F_k2
+    a0 = __dadd_rn(__fma_rn(M[1], x.y, __dmul_rn(M[0], x.x)), M[2]);
+    a1 = __dadd_rn(__fma_rn(M[4], x.y, __dmul_rn(M[3], x.x)), M[5]);
+    a2 = __dadd_rn(__fma_rn(M[7], x.y, __dmul_rn(M[6], x.x)), M[8]);
+    n = __dadd_rn(__dmul_rn(a0, a0), __dmul_rn(a1, a1));
+  } else {                                                         // H x: fma(H_k0, x, H_k1 y) + H_k2
+    const double p0 = __dadd_rn(__fma_rn(M[0], x.x, __dmul_rn(M[1], x.y)), M[2]);
+    const double p1 = __dadd_rn(__fma_rn(M[3], x.x, __dmul_rn(M[4], x.y)), M[5]);
+    const double p2 = __dadd_rn(__fma_rn(M[6], x.x, __dmul_rn(M[7], x.y)), M[8]);
+    a0 = __ddiv_rn(p0, p2); a1 = __ddiv_rn(p1, p2);
+  }
+  uint4 qd[8];
+  int qn = 0;
+  if (DESC) {
+    const uint4 *qp = reinterpret_cast<const uint4 *>(desc + (size_t)(P.q_row0 + (active ? i : 0)) * OMVG_DESC_LEN);
+    #pragma unroll
+    for (int k = 0; k < 8; ++k) qd[k] = qp[k];
+    qn = norm[P.q_row0 + (active ? i : 0)];
+  }
+  int bd = INT_MAX, sbd = INT_MAX;                                 // integer distances < 2^23: INT_MAX = "none yet"
+  double emin = DBL_MAX;
+  uint32_t idx = 0;
+  for (uint32_t j0 = 0; j0 < P.db_count; j0 += GM_CHUNK) {
+    const uint32_t nj = min((uint32_t)GM_CHUNK, P.db_count - j0);
+    __syncthreads();
+    for (uint32_t t = threadIdx.x; t < nj; t += GM_THREADS) sj[t] = pos[P.db_row0 + j0 + t];
+    __syncthreads();
+    if (!active) continue;
+    for (uint32_t t = 0; t < nj; ++t) {
+      const double2 y = sj[t];
+      double err;
+      if (MODEL == OMVG_GUIDED_EPIPOLAR) {
+        const double dt = __dadd_rn(__dadd_rn(__dmul_rn(a0, y.x), __dmul_rn(a1, y.y)), a2);
+        err = __ddiv_rn(__dmul_rn(dt, dt), n);
+      } else {
+        const double dx = __dsub_rn(y.x, a0), dy = __dsub_rn(y.y, a1);
+        err = __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy));
+      }
+      if (!(err < thr)) continue;
+      if (DESC) {
+        const uint32_t r = P.db_row0 + j0 + t;
+        const uint4 *rp = reinterpret_cast<const uint4 *>(desc + (size_t)r * OMVG_DESC_LEN);
+        uint32_t dot = 0;
+        #pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          const uint4 v = rp[k];
+          dot = __dp4a(v.x, qd[k].x, dot); dot = __dp4a(v.y, qd[k].y, dot);
+          dot = __dp4a(v.z, qd[k].z, dot); dot = __dp4a(v.w, qd[k].w, dot);
+        }
+        const int d = qn + norm[r] - 2 * (int)dot;
+        if (d < bd) { idx = j0 + t; sbd = bd; bd = d; } else if (d < sbd) sbd = d;   // guided_matching.hpp:86-102
+      } else if (err < emin) { emin = err; idx = j0 + t; }
+    }
+  }
+  if (!active) return;
+  const bool keep = DESC ? sbd != INT_MAX && __int2double_rn(bd) < __dmul_rn(ratio, __int2double_rn(sbd))   // :105-112
+                         : emin < thr;
+  out[P.out_off + i].x = keep ? (int)idx : -1;
+}
+
+// ordered compaction of one pair's guided results: (i, j) for the matched i, ascending i
+__global__ void __launch_bounds__(FIN_THREADS) guided_compact_kernel(const PairInfo *__restrict__ pairs, int2 *__restrict__ k12, uint32_t *__restrict__ counts) {
+  __shared__ uint32_t warp_tot[FIN_THREADS / 32];
+  __shared__ uint32_t running;
+  const PairInfo P = pairs[blockIdx.x];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) running = 0;
+  __syncthreads();
+  int2 *io = k12 + P.out_off;
+  for (uint32_t q0 = 0; q0 < P.q_count; q0 += FIN_THREADS) {
+    const uint32_t q = q0 + threadIdx.x;
+    const int v = q < P.q_count ? io[q].x : -1;
+    const bool keep = v >= 0;
+    const uint32_t bal = __ballot_sync(0xffffffffu, keep);
+    const uint32_t in_warp = __popc(bal & ((1u << lane) - 1));
+    if (lane == 0) warp_tot[warp] = __popc(bal);
+    __syncthreads();
+    uint32_t before = running;
+    for (int w = 0; w < warp; ++w) before += warp_tot[w];
+    if (keep) reinterpret_cast<uint2 *>(io)[before + in_warp] = make_uint2(q, (uint32_t)v);
+    __syncthreads();
+    if (threadIdx.x == 0) { uint32_t t = 0; for (int w = 0; w < FIN_THREADS / 32; ++w) t += warp_tot[w]; running += t; }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) counts[blockIdx.x] = running;
+}
+
 }  // namespace omvg
 
 // ===================================================================================== host side
@@ -745,6 +865,9 @@ struct omvg_match_ctx {
   // cascade hashing state (omvg_match_cascade_prepare)
   uint4 *d_code = nullptr, *d_bid = nullptr; uint32_t *d_bstart = nullptr, *d_bitems = nullptr; float *d_proj = nullptr, *d_zm = nullptr;
   bool cascade_ready = false; std::vector<float> h_zm;
+  // guided matching (omvg_match_upload_positions / omvg_match_guided_run): one double2 per arena row
+  double2 *d_pos = nullptr; std::vector<uint8_t> has_pos;
+  GuidedModel *d_models = nullptr; size_t models_cap = 0;
 };
 
 namespace {
@@ -782,6 +905,7 @@ void free_images(omvg_match_ctx *c) {
   cudaFree(c->d_img_group); cudaFree(c->d_row_img); cudaFree(c->d_dig); cudaFree(c->d_img_c0); cudaFree(c->d_hmm);
   c->d_dig = nullptr; c->d_img_c0 = nullptr; c->d_hmm = nullptr; c->use_dig = false;
   c->d_desc = nullptr; c->d_norm = c->d_ckey = nullptr; c->d_img_row0 = c->d_img_count = c->d_img_group = c->d_row_img = nullptr;
+  cudaFree(c->d_pos); c->d_pos = nullptr; c->has_pos.clear();
 }
 
 template <typename T> int ensure(T *&p, size_t &cap, size_t need) {
@@ -802,6 +926,53 @@ int drain_timers(omvg_match_ctx *c) {
 cudaEvent_t get_event(omvg_match_ctx *c) {
   if (!c->ev_pool.empty()) { cudaEvent_t e = c->ev_pool.back(); c->ev_pool.pop_back(); return e; }
   cudaEvent_t e; cudaEventCreate(&e); return e;
+}
+
+// per-pair device table of one batch (d_pairs / d_counts), grown on demand
+int ensure_pairs(omvg_match_ctx *c, uint32_t nb) {
+  if (nb <= c->pairs_cap) return OMVG_OK;
+  if (c->d_pairs) cudaFree(c->d_pairs); if (c->d_counts) cudaFree(c->d_counts);
+  c->d_pairs = nullptr; c->d_counts = nullptr; c->pairs_cap = 0;
+  OMVG_CUDA(cudaMalloc(&c->d_pairs, nb * sizeof(PairInfo))); OMVG_CUDA(cudaMalloc(&c->d_counts, nb * sizeof(uint32_t)));
+  c->pairs_cap = nb; return OMVG_OK;
+}
+
+// a new CSR result over n_pairs pairs: offsets[0] = 0, running total 0
+int begin_result(omvg_match_ctx *c, uint64_t n_pairs) {
+  if (n_pairs + 1 > c->offsets_cap) {
+    if (c->d_offsets) cudaFree(c->d_offsets);
+    c->d_offsets = nullptr; c->offsets_cap = 0;
+    OMVG_CUDA(cudaMalloc(&c->d_offsets, (n_pairs + 1) * sizeof(uint64_t))); c->offsets_cap = n_pairs + 1;
+  }
+  OMVG_CUDA(cudaMemsetAsync(c->d_total, 0, sizeof(uint64_t), c->stream));
+  OMVG_CUDA(cudaMemsetAsync(c->d_offsets, 0, sizeof(uint64_t), c->stream));
+  c->total_last = 0; c->n_pairs_last = n_pairs; c->have_result = false;
+  return OMVG_OK;
+}
+
+// the per-pair counts of batch [p0, p0 + nb) are in d_counts and each pair's rows sit compacted at the start of its
+// d_k12 segment: scan the counts into the global offsets and append the rows to d_out
+int gather_batch(omvg_match_ctx *c, uint32_t nb, uint64_t p0) {
+  scan_counts_kernel<<<1, 1024, 0, c->stream>>>(c->d_counts, nb, c->d_offsets + p0, c->d_total);
+  OMVG_CUDA(cudaGetLastError());
+  c->launches++;
+  // size the global output buffer: needs the running total (one small sync per batch)
+  uint64_t total = 0;
+  OMVG_CUDA(cudaMemcpyAsync(&total, c->d_total, sizeof total, cudaMemcpyDeviceToHost, c->stream));
+  OMVG_CUDA(cudaStreamSynchronize(c->stream));
+  if (total > c->out_cap) {
+    const size_t ncap = std::max<size_t>(total, c->out_cap * 2 + 1024);
+    uint2 *n = nullptr; OMVG_CUDA(cudaMalloc(&n, ncap * sizeof(uint2)));
+    if (c->d_out && c->total_last) OMVG_CUDA(cudaMemcpyAsync(n, c->d_out, c->total_last * sizeof(uint2), cudaMemcpyDeviceToDevice, c->stream));
+    OMVG_CUDA(cudaStreamSynchronize(c->stream));
+    if (c->d_out) cudaFree(c->d_out);
+    c->d_out = n; c->out_cap = ncap;
+  }
+  compact_kernel<<<nb, 128, 0, c->stream>>>(c->d_k12, c->d_pairs, c->d_counts, c->d_offsets + p0, c->d_out);
+  OMVG_CUDA(cudaGetLastError());
+  c->launches++;
+  c->total_last = total;
+  return OMVG_OK;
 }
 
 // one batch of pairs: tensor-core kernel + finalize + scan + compact
@@ -827,12 +998,7 @@ int run_batch(omvg_match_ctx *c, const uint32_t *pi, const uint32_t *pj, uint64_
   int rc;
   if ((rc = ensure(c->d_k12, c->k12_cap, std::max<size_t>(out, 1)))) return rc;
   if ((rc = ensure(c->d_units, c->units_cap, std::max<size_t>(n_units, 1)))) return rc;
-  if (nb > c->pairs_cap) {
-    if (c->d_pairs) cudaFree(c->d_pairs); if (c->d_counts) cudaFree(c->d_counts);
-    c->d_pairs = nullptr; c->d_counts = nullptr; c->pairs_cap = 0;
-    OMVG_CUDA(cudaMalloc(&c->d_pairs, nb * sizeof(PairInfo))); OMVG_CUDA(cudaMalloc(&c->d_counts, nb * sizeof(uint32_t)));
-    c->pairs_cap = nb;
-  }
+  if ((rc = ensure_pairs(c, nb))) return rc;
   OMVG_CUDA(cudaMemcpyAsync(c->d_pairs, pinfo.data(), nb * sizeof(PairInfo), cudaMemcpyHostToDevice, c->stream));
   if (n_units) {
     expand_units_kernel<<<nb, 64, 0, c->stream>>>(c->d_pairs, c->d_units); OMVG_CUDA(cudaGetLastError()); c->launches++;
@@ -848,26 +1014,8 @@ int run_batch(omvg_match_ctx *c, const uint32_t *pi, const uint32_t *pj, uint64_
   if (c->use_dig) match_finalize_kernel<true><<<nb, FIN_THREADS, 0, c->stream>>>(c->d_desc, c->d_norm, c->d_pairs, c->d_k12, c->d_counts, fratio);
   else match_finalize_kernel<false><<<nb, FIN_THREADS, 0, c->stream>>>(c->d_desc, c->d_norm, c->d_pairs, c->d_k12, c->d_counts, fratio);
   OMVG_CUDA(cudaGetLastError());
-  scan_counts_kernel<<<1, 1024, 0, c->stream>>>(c->d_counts, nb, c->d_offsets + p0, c->d_total);
-  OMVG_CUDA(cudaGetLastError());
-  c->launches += 2;
-  // size the global output buffer: needs the running total (one small sync per batch)
-  uint64_t total = 0;
-  OMVG_CUDA(cudaMemcpyAsync(&total, c->d_total, sizeof total, cudaMemcpyDeviceToHost, c->stream));
-  OMVG_CUDA(cudaStreamSynchronize(c->stream));
-  if (total > c->out_cap) {
-    const size_t ncap = std::max<size_t>(total, c->out_cap * 2 + 1024);
-    uint2 *n = nullptr; OMVG_CUDA(cudaMalloc(&n, ncap * sizeof(uint2)));
-    if (c->d_out && c->total_last) OMVG_CUDA(cudaMemcpyAsync(n, c->d_out, c->total_last * sizeof(uint2), cudaMemcpyDeviceToDevice, c->stream));
-    OMVG_CUDA(cudaStreamSynchronize(c->stream));
-    if (c->d_out) cudaFree(c->d_out);
-    c->d_out = n; c->out_cap = ncap;
-  }
-  compact_kernel<<<nb, 128, 0, c->stream>>>(c->d_k12, c->d_pairs, c->d_counts, c->d_offsets + p0, c->d_out);
-  OMVG_CUDA(cudaGetLastError());
   c->launches++;
-  c->total_last = total;
-  return OMVG_OK;
+  return gather_batch(c, nb, p0);
 }
 
 }  // namespace
@@ -907,7 +1055,7 @@ int omvg_match_destroy(omvg_match_ctx *c) {
   drain_timers(c); for (auto e : c->ev_pool) cudaEventDestroy(e);
   free_images(c);
   cudaFree(c->d_k12); cudaFree(c->d_units); cudaFree(c->d_pairs); cudaFree(c->d_counts); cudaFree(c->d_offsets);
-  cudaFree(c->d_total); cudaFree(c->d_out);
+  cudaFree(c->d_total); cudaFree(c->d_out); cudaFree(c->d_models);
   if (c->h_offsets) cudaFreeHost(c->h_offsets); if (c->h_ij) cudaFreeHost(c->h_ij);
   cudaStreamDestroy(c->stream);
   delete c; return OMVG_OK;
@@ -1018,14 +1166,7 @@ int omvg_match_run(omvg_match_ctx *c, const uint32_t *pair_i, const uint32_t *pa
   for (uint64_t p = 0; p < n_pairs; ++p)
     if (pair_i[p] >= c->n_images || pair_j[p] >= c->n_images) return fail(OMVG_E_ARG, "pair %llu out of range", (unsigned long long)p);
   const float fratio = dist_ratio * dist_ratio;                   // numeric.h:56 Square<float>, regions_matcher.hpp:196
-  if (n_pairs + 1 > c->offsets_cap) {
-    if (c->d_offsets) cudaFree(c->d_offsets);
-    c->d_offsets = nullptr; c->offsets_cap = 0;
-    OMVG_CUDA(cudaMalloc(&c->d_offsets, (n_pairs + 1) * sizeof(uint64_t))); c->offsets_cap = n_pairs + 1;
-  }
-  OMVG_CUDA(cudaMemsetAsync(c->d_total, 0, sizeof(uint64_t), c->stream));
-  OMVG_CUDA(cudaMemsetAsync(c->d_offsets, 0, sizeof(uint64_t), c->stream));
-  c->total_last = 0; c->n_pairs_last = n_pairs; c->have_result = false;
+  if (const int rc = begin_result(c, n_pairs)) return rc;
   std::vector<Unit> units; std::vector<PairInfo> pinfo;
   const size_t budget = c->k12_budget_bytes / sizeof(int2);
   uint64_t p0 = 0;
@@ -1148,14 +1289,7 @@ int omvg_match_cascade_run(omvg_match_ctx *c, const uint32_t *pair_i, const uint
   for (uint64_t p = 0; p < n_pairs; ++p)
     if (pair_i[p] >= c->n_images || pair_j[p] >= c->n_images) return fail(OMVG_E_ARG, "pair %llu out of range", (unsigned long long)p);
   const float fratio = dist_ratio * dist_ratio;
-  if (n_pairs + 1 > c->offsets_cap) {
-    if (c->d_offsets) cudaFree(c->d_offsets);
-    c->d_offsets = nullptr; c->offsets_cap = 0;
-    OMVG_CUDA(cudaMalloc(&c->d_offsets, (n_pairs + 1) * sizeof(uint64_t))); c->offsets_cap = n_pairs + 1;
-  }
-  OMVG_CUDA(cudaMemsetAsync(c->d_total, 0, sizeof(uint64_t), c->stream));
-  OMVG_CUDA(cudaMemsetAsync(c->d_offsets, 0, sizeof(uint64_t), c->stream));
-  c->total_last = 0; c->n_pairs_last = n_pairs; c->have_result = false;
+  if (const int rc = begin_result(c, n_pairs)) return rc;
   std::vector<PairInfo> pinfo;
   const size_t budget = c->k12_budget_bytes / sizeof(int2);
   uint64_t p0 = 0;
@@ -1171,12 +1305,7 @@ int omvg_match_cascade_run(omvg_match_ctx *c, const uint32_t *pair_i, const uint
     const uint32_t nb = (uint32_t)(p1 - p0);
     int rc;
     if ((rc = ensure(c->d_k12, c->k12_cap, std::max<size_t>(out, 1)))) return rc;
-    if (nb > c->pairs_cap) {
-      if (c->d_pairs) cudaFree(c->d_pairs); if (c->d_counts) cudaFree(c->d_counts);
-      c->d_pairs = nullptr; c->d_counts = nullptr; c->pairs_cap = 0;
-      OMVG_CUDA(cudaMalloc(&c->d_pairs, nb * sizeof(PairInfo))); OMVG_CUDA(cudaMalloc(&c->d_counts, nb * sizeof(uint32_t)));
-      c->pairs_cap = nb;
-    }
+    if ((rc = ensure_pairs(c, nb))) return rc;
     OMVG_CUDA(cudaMemcpyAsync(c->d_pairs, pinfo.data(), nb * sizeof(PairInfo), cudaMemcpyHostToDevice, c->stream));
     if (maxq) {
       cudaEvent_t e0 = get_event(c), e1 = get_event(c);
@@ -1187,21 +1316,79 @@ int omvg_match_cascade_run(omvg_match_ctx *c, const uint32_t *pair_i, const uint
       c->pending.emplace_back(e0, e1); c->tc_launches++; c->launches++;
     }
     cascade_compact_kernel<<<nb, FIN_THREADS, 0, c->stream>>>(c->d_pairs, c->d_k12, c->d_counts); OMVG_CUDA(cudaGetLastError());
-    scan_counts_kernel<<<1, 1024, 0, c->stream>>>(c->d_counts, nb, c->d_offsets + p0, c->d_total); OMVG_CUDA(cudaGetLastError());
-    c->launches += 2;
-    uint64_t total = 0;
-    OMVG_CUDA(cudaMemcpyAsync(&total, c->d_total, sizeof total, cudaMemcpyDeviceToHost, c->stream));
-    OMVG_CUDA(cudaStreamSynchronize(c->stream));
-    if (total > c->out_cap) {
-      const size_t ncap = std::max<size_t>(total, c->out_cap * 2 + 1024);
-      uint2 *n = nullptr; OMVG_CUDA(cudaMalloc(&n, ncap * sizeof(uint2)));
-      if (c->d_out && c->total_last) OMVG_CUDA(cudaMemcpyAsync(n, c->d_out, c->total_last * sizeof(uint2), cudaMemcpyDeviceToDevice, c->stream));
-      OMVG_CUDA(cudaStreamSynchronize(c->stream));
-      if (c->d_out) cudaFree(c->d_out);
-      c->d_out = n; c->out_cap = ncap;
+    c->launches++;
+    if ((rc = gather_batch(c, nb, p0))) return rc;
+    p0 = p1;
+  }
+  c->have_result = true; return OMVG_OK;
+}
+
+// ---- guided matching ---------------------------------------------------------------------------------------
+int omvg_match_upload_positions(omvg_match_ctx *c, uint32_t image, const double *xy) {
+  if (!c) return fail(OMVG_E_ARG, "null ctx");
+  if (!c->d_desc) return fail(OMVG_E_STATE, "set_images first");
+  if (image >= c->n_images || (!xy && c->counts[image])) return fail(OMVG_E_ARG, "bad image %u", image);
+  OMVG_CUDA(cudaSetDevice(c->device));
+  if (!c->d_pos) {
+    OMVG_CUDA(cudaMalloc(&c->d_pos, (size_t)c->total_rows * sizeof(double2)));
+    c->has_pos.assign(c->n_images, 0);
+  }
+  if (c->counts[image])
+    OMVG_CUDA(cudaMemcpyAsync(c->d_pos + c->row0[image], xy, (size_t)c->counts[image] * sizeof(double2), cudaMemcpyHostToDevice, c->stream));
+  c->has_pos[image] = 1;
+  return OMVG_OK;
+}
+
+// GuidedMatching for pairs (I = pair_i[p], J = pair_j[p]); fetch with omvg_match_fetch: rows of (i, j), ascending i.
+int omvg_match_guided_run(omvg_match_ctx *c, int32_t error_model, const uint32_t *pair_i, const uint32_t *pair_j, uint64_t n_pairs,
+                          const double *models, const double *thresholds, double dist_ratio) {
+  if (!c || ((!pair_i || !pair_j || !models || !thresholds) && n_pairs)) return fail(OMVG_E_ARG, "bad arguments");
+  if (error_model != OMVG_GUIDED_EPIPOLAR && error_model != OMVG_GUIDED_TRANSFER) return fail(OMVG_E_ARG, "unknown error model %d", error_model);
+  if (std::isnan(dist_ratio)) return fail(OMVG_E_ARG, "dist_ratio is NaN");
+  if (!c->prepared) return fail(OMVG_E_STATE, "omvg_match_prepare must follow the uploads");
+  for (uint64_t p = 0; p < n_pairs; ++p) {
+    if (pair_i[p] >= c->n_images || pair_j[p] >= c->n_images) return fail(OMVG_E_ARG, "pair %llu out of range", (unsigned long long)p);
+    if (c->has_pos.empty() || !c->has_pos[pair_i[p]] || !c->has_pos[pair_j[p]]) return fail(OMVG_E_STATE, "pair %llu: an image has no positions", (unsigned long long)p);
+    bool finite = std::isfinite(thresholds[p]);
+    for (int k = 0; k < 9; ++k) finite = finite && std::isfinite(models[9 * p + k]);
+    if (!finite) return fail(OMVG_E_ARG, "pair %llu: non-finite model or threshold", (unsigned long long)p);
+  }
+  OMVG_CUDA(cudaSetDevice(c->device));
+  if (const int rc = begin_result(c, n_pairs)) return rc;
+  const bool desc = dist_ratio >= 0.0;
+  std::vector<PairInfo> pinfo; std::vector<GuidedModel> gm;
+  const size_t budget = c->k12_budget_bytes / sizeof(int2);
+  uint64_t p0 = 0;
+  while (p0 < n_pairs) {
+    pinfo.clear(); gm.clear(); size_t out = 0; uint64_t p1 = p0; uint32_t maxq = 0;
+    while (p1 < n_pairs && p1 - p0 < 65535) {
+      const uint32_t I = pair_i[p1], J = pair_j[p1];
+      if (p1 > p0 && out + c->counts[I] > budget) break;
+      PairInfo P{}; P.q_row0 = c->row0[I]; P.q_count = c->counts[I]; P.db_row0 = c->row0[J]; P.db_count = c->counts[J]; P.out_off = out;
+      GuidedModel G; for (int k = 0; k < 9; ++k) G.M[k] = models[9 * p1 + k]; G.thr = thresholds[p1];
+      out += P.q_count; maxq = std::max(maxq, P.q_count); pinfo.push_back(P); gm.push_back(G); ++p1;
     }
-    compact_kernel<<<nb, 128, 0, c->stream>>>(c->d_k12, c->d_pairs, c->d_counts, c->d_offsets + p0, c->d_out); OMVG_CUDA(cudaGetLastError());
-    c->launches++; c->total_last = total;
+    const uint32_t nb = (uint32_t)(p1 - p0);
+    int rc;
+    if ((rc = ensure(c->d_k12, c->k12_cap, std::max<size_t>(out, 1)))) return rc;
+    if ((rc = ensure_pairs(c, nb))) return rc;
+    if ((rc = ensure(c->d_models, c->models_cap, nb))) return rc;
+    OMVG_CUDA(cudaMemcpyAsync(c->d_pairs, pinfo.data(), nb * sizeof(PairInfo), cudaMemcpyHostToDevice, c->stream));
+    OMVG_CUDA(cudaMemcpyAsync(c->d_models, gm.data(), nb * sizeof(GuidedModel), cudaMemcpyHostToDevice, c->stream));
+    if (maxq) {
+      const dim3 grid((maxq + GM_THREADS - 1) / GM_THREADS, nb);
+      cudaEvent_t e0 = get_event(c), e1 = get_event(c);
+      OMVG_CUDA(cudaEventRecord(e0, c->stream));
+      auto k = error_model == OMVG_GUIDED_EPIPOLAR ? (desc ? guided_match_kernel<OMVG_GUIDED_EPIPOLAR, true> : guided_match_kernel<OMVG_GUIDED_EPIPOLAR, false>)
+                                                   : (desc ? guided_match_kernel<OMVG_GUIDED_TRANSFER, true> : guided_match_kernel<OMVG_GUIDED_TRANSFER, false>);
+      k<<<grid, GM_THREADS, 0, c->stream>>>(c->d_pos, c->d_desc, c->d_norm, c->d_pairs, c->d_models, c->d_k12, dist_ratio);
+      OMVG_CUDA(cudaGetLastError());
+      OMVG_CUDA(cudaEventRecord(e1, c->stream));
+      c->pending.emplace_back(e0, e1); c->tc_launches++; c->launches++;
+    }
+    guided_compact_kernel<<<nb, FIN_THREADS, 0, c->stream>>>(c->d_pairs, c->d_k12, c->d_counts); OMVG_CUDA(cudaGetLastError());
+    c->launches++;
+    if ((rc = gather_batch(c, nb, p0))) return rc;
     p0 = p1;
   }
   c->have_result = true; return OMVG_OK;

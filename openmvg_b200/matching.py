@@ -16,6 +16,7 @@ import numpy as np
 from ._lib import check, lib
 
 _vp = ctypes.c_void_p
+GUIDED_EPIPOLAR, GUIDED_TRANSFER = 0, 1          # OMVG_GUIDED_EPIPOLAR (F, or F from E), OMVG_GUIDED_TRANSFER (H)
 
 
 def _p(a):
@@ -104,6 +105,24 @@ class MatchContext:
         ms = ctypes.c_double(); n = ctypes.c_uint64()
         check(lib().omvg_match_kernel_time(self._h, ctypes.byref(ms), ctypes.byref(n), int(reset)))
         return ms.value, n.value
+
+    # ---- guided matching (geometry_aware::GuidedMatching; the -r step of the geometric filter)
+    def upload_positions(self, image: int, xy):
+        """Feature positions [counts[image], 2] in pixels (undistorted when the view has an intrinsic)."""
+        xy = np.ascontiguousarray(xy, np.float64)
+        assert xy.size == int(self.counts[image]) * 2
+        check(lib().omvg_match_upload_positions(self._h, int(image), _p(xy)))
+
+    def guided_run(self, pair_i, pair_j, models, thresholds, dist_ratio: float, error_model: int = GUIDED_EPIPOLAR):
+        """models [n,3,3] (image pair_i -> image pair_j), thresholds [n] (err < thr), dist_ratio already squared
+        (< 0: the descriptor-free variant); error_model 0 = epipolar (F), 1 = transfer (H).  Read with fetch():
+        rows of (i in pair_i, j in pair_j), ascending i."""
+        self._pi = np.ascontiguousarray(pair_i, np.uint32)
+        self._pj = np.ascontiguousarray(pair_j, np.uint32)
+        M = np.ascontiguousarray(models, np.float64).reshape(len(self._pi), 9)
+        t = np.ascontiguousarray(thresholds, np.float64).reshape(len(self._pi))
+        check(lib().omvg_match_guided_run(self._h, ctypes.c_int32(error_model), _p(self._pi), _p(self._pj),
+                                          ctypes.c_uint64(len(self._pi)), _p(M), _p(t), ctypes.c_double(dist_ratio)))
 
     # ---- validation aids
     # ---- cascade hashing (FASTCASCADEHASHINGL2; Cascade_Hashing_Matcher_Regions.cpp)

@@ -297,3 +297,76 @@ def calibrated_two_view_matches(n: int, outlier_frac: float = 0.3, seed: int = 3
     xJ[out] = np.stack([rng.uniform(0, w, int(out.sum())), rng.uniform(0, h, int(out.sum()))], 1)
     return (xI.astype(np.float32).astype(np.float64), xJ.astype(np.float32).astype(np.float64), ~out,
             tuple(float(v) for v in intr_I), tuple(float(v) for v in intr_J))
+
+
+def guided_scene(n_views: int, n_feat, seed: int = 9, wh=(1600, 1200), planar: bool = False, shared_frac: float = 0.6,
+                 n_dup: int = 0, desc_noise: int = 8, noise_px: float = 0.5):
+    """Per-view feature positions and SIFT-like descriptors of one 3-D scene for guided matching (DESIGN §3.9).
+    n_feat: features per view (int or list).  About shared_frac of each view's features are projections of shared
+    3-D points (one base descriptor per point, +-desc_noise per view, 0.5 px position noise); the rest are distractors
+    with their own random descriptors and positions.  planar: the points lie on one plane (homography scenes).
+    n_dup: that many features per view repeat the position of another feature of the view (different descriptor).
+    Views look at the scene from a short arc with different pinhole intrinsics; feature order is shuffled.
+    Positions are float32 values (openMVG keeps feature coordinates in float).
+    -> dict xy [list of [n,2] float64], desc [list of [n,128] uint8], point [list of [n] int, -1 = distractor],
+       K [list of 3x3], R, C [lists], plane (n, d) or None, wh."""
+    rng = np.random.default_rng(seed)
+    w, h = wh
+    counts = [int(n_feat)] * n_views if np.isscalar(n_feat) else [int(v) for v in n_feat]
+    n_pts = max(1, int(shared_frac * max(counts + [1]) * 1.6))
+    X = np.stack([rng.uniform(-2.0, 2.0, n_pts), rng.uniform(-1.5, 1.5, n_pts), rng.uniform(5.0, 9.0, n_pts)], 1)
+    plane = None
+    if planar:
+        nrm = np.array([0.1, -0.15, 1.0]); nrm /= np.linalg.norm(nrm)
+        plane = (nrm, 7.0)
+        X[:, 2] = (7.0 - nrm[0] * X[:, 0] - nrm[1] * X[:, 1]) / nrm[2]
+    base = rng.integers(0, 140, (n_pts, 128), dtype=np.int32)
+    Ks, Rs, Cs, xys, descs, pids = [], [], [], [], [], []
+    for v in range(n_views):
+        f = max(w, h) * (0.9 + 0.25 * rng.random())
+        K = np.array([[f, 0, w / 2 + rng.uniform(-20, 20)], [0, f, h / 2 + rng.uniform(-20, 20)], [0, 0, 1.0]])
+        ang = 0.35 * (v / max(1, n_views - 1) - 0.5)
+        C = np.array([7.0 * np.sin(ang), 0.2 * rng.normal(), 7.0 - 7.0 * np.cos(ang)])
+        R = _rodrigues(np.array([0.02 * rng.normal(), -ang, 0.02 * rng.normal()]))
+        Xc = (X - C) @ R.T
+        uv = np.stack([K[0, 2] + f * Xc[:, 0] / Xc[:, 2], K[1, 2] + f * Xc[:, 1] / Xc[:, 2]], 1) + rng.normal(0, noise_px, (n_pts, 2))
+        vis = np.flatnonzero((Xc[:, 2] > 0) & (uv[:, 0] >= 0) & (uv[:, 0] < w) & (uv[:, 1] >= 0) & (uv[:, 1] < h))
+        n = counts[v]
+        ns = min(len(vis), int(round(shared_frac * n)), n)
+        sel = rng.choice(vis, ns, replace=False) if ns else np.zeros(0, np.int64)
+        nd = n - ns
+        xy = np.concatenate([uv[sel], np.stack([rng.uniform(0, w, nd), rng.uniform(0, h, nd)], 1)])
+        d = np.concatenate([base[sel] + rng.integers(-desc_noise, desc_noise + 1, (ns, 128)), rng.integers(0, 140, (nd, 128))])
+        pid = np.concatenate([sel, -np.ones(nd, np.int64)])
+        perm = rng.permutation(n)
+        xy, d, pid = xy[perm], d[perm], pid[perm]
+        if n_dup and n > 1:
+            src = rng.choice(n, min(n_dup, n - 1), replace=False)
+            dst = (src + 1 + rng.integers(0, n - 1, len(src))) % n
+            xy[dst] = xy[src]
+        Ks.append(K); Rs.append(R); Cs.append(C)
+        xys.append(xy.astype(np.float32).astype(np.float64))
+        descs.append(np.clip(d, 0, 255).astype(np.uint8))
+        pids.append(pid)
+    return dict(xy=xys, desc=descs, point=pids, K=Ks, R=Rs, C=Cs, plane=plane, wh=(w, h))
+
+
+def scene_fundamental(scene: dict, a: int, b: int) -> np.ndarray:
+    """F with x_b^T F x_a = 0 for the views a, b of guided_scene (the epipolar line of x_a in view b is F x_a)."""
+    R = scene["R"][b] @ scene["R"][a].T
+    t = scene["R"][b] @ (scene["C"][a] - scene["C"][b])
+    tx = np.array([[0, -t[2], t[1]], [t[2], 0, -t[0]], [-t[1], t[0], 0]])
+    F = np.linalg.inv(scene["K"][b]).T @ tx @ R @ np.linalg.inv(scene["K"][a])
+    return F / np.linalg.norm(F)
+
+
+def scene_homography(scene: dict, a: int, b: int) -> np.ndarray:
+    """The homography x_b ~ H x_a induced by the plane of a planar guided_scene (by the plane at infinity otherwise)."""
+    R = scene["R"][b] @ scene["R"][a].T
+    G = R
+    if scene["plane"] is not None:
+        nrm, d = scene["plane"]
+        t = scene["R"][b] @ (scene["C"][a] - scene["C"][b])
+        G = R + np.outer(t, scene["R"][a] @ nrm) / (d - nrm @ scene["C"][a])
+    H = scene["K"][b] @ G @ np.linalg.inv(scene["K"][a])
+    return H / H[2, 2]
