@@ -342,6 +342,17 @@ int omvg_ba_commit(omvg_ba_ctx *ctx);
  * Huber-corrected, NOT Jacobi-scaled), in the caller's observation order; cost returned. */
 int omvg_ba_debug_eval(omvg_ba_ctx *ctx, const omvg_ba_options *options, double *cost, double *r,
                        double *J_intr, double *J_pose, double *J_point);
+/* Validation aid (tests only): the first LM step of omvg_ba_run at trust-region radius `radius`, taken apart.  With
+ * nd = 6 n_poses + 8 n_intrinsics and nx = 3 n_points + nd (points, then poses, then intrinsic slots):
+ *   scale[nx]      Jacobi column scaling of the unscaled J;  lm_diag[nx]  LM diagonal D (D^2 = clamp(diag) / radius)
+ *   S[nd][nd]      reduced system as the solver sees it (D^2 included, constant coordinates as identity rows), row-major
+ *   rhs[nd], z[nd] its right-hand side and the solver's output;  step_point[n_points][3]  back-substituted landmark step
+ *   model_change   model cost change of the step;  solver  0 dense L D L', 1 explicit inverse, 2 pcg5, 3 pcg3, 4 pcg
+ *   pcg_stats[3]   iterations, relative residual the PCG reported, |rhs| (zeros on the direct paths)
+ * All in the caller's pose / intrinsic / landmark order; any pointer may be NULL.  The parameters are not changed. */
+int omvg_ba_debug_step(omvg_ba_ctx *ctx, const omvg_ba_options *options, double radius, double *scale, double *lm_diag,
+                       double *S, double *rhs, double *z, double *step_point, double *model_change, int32_t *solver,
+                       double *pcg_stats);
 
 #ifdef __cplusplus
 }

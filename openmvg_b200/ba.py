@@ -194,6 +194,25 @@ class BAContext:
         check(lib().omvg_ba_debug_eval(self._h, ctypes.byref(o), ctypes.byref(cost), d(r), d(Ji), d(Jc), d(Jp)))
         return cost.value, r, Ji, Jc, Jp
 
+    # solver ids of omvg_ba_debug_step
+    SOLVERS = ("dense_ldlt", "dense_inverse", "pcg5", "pcg3", "pcg")
+
+    def debug_step(self, radius: float, **opts) -> dict:
+        """The first LM step of run() at trust-region radius `radius`, stage by stage (omvg_ba_debug_step): Jacobi
+        scaling, LM diagonal, the dense reduced system S and its right-hand side, the solver's z, the landmark step and
+        the model cost change.  Vectors over all columns are ordered points (3 n_points), poses (6 n_poses), intrinsic
+        slots (8 n_intrinsics); S, rhs and z cover the last two."""
+        o = default_options(**opts)
+        npt, nc, ni = len(self._keep[2]), len(self._keep[0]), len(self._keep[1])
+        nd = 6 * nc + 8 * ni; nx = 3 * npt + nd
+        scale = np.zeros(nx); lm = np.zeros(nx); S = np.zeros((nd, nd)); rhs = np.zeros(nd); z = np.zeros(nd)
+        step = np.zeros((npt, 3)); model = ctypes.c_double(); solver = ctypes.c_int32(); pcg = np.zeros(3)
+        d = lambda a: a.ctypes.data_as(_dp)   # noqa: E731
+        check(lib().omvg_ba_debug_step(self._h, ctypes.byref(o), ctypes.c_double(radius), d(scale), d(lm), d(S), d(rhs), d(z), d(step),
+                                       ctypes.byref(model), ctypes.byref(solver), d(pcg)))
+        return dict(scale=scale, lm_diag=lm, S=S, rhs=rhs, z=z, step_point=step, model_change=model.value,
+                    solver=self.SOLVERS[solver.value], pcg_iterations=int(pcg[0]), pcg_relres=pcg[1], pcg_bnorm=pcg[2])
+
 
 class Bundle_Adjustment_B200:
     """Drop-in for Bundle_Adjustment_Ceres on the flat scene: Adjust(scene, options) -> bool, scene

@@ -1204,4 +1204,60 @@ int omvg_ba_debug_eval(omvg_ba_ctx *c, const omvg_ba_options *O, double *cost, d
   return OMVG_OK;
 }
 
+// The phases of omvg_ba_run's first LM step, by the same functions; the reduced system is read back before the solve
+int omvg_ba_debug_step(omvg_ba_ctx *c, const omvg_ba_options *O, double radius, double *scale, double *lm_diag, double *S, double *rhs, double *z,
+                       double *step_point, double *model_change, int32_t *solver, double *pcg_stats) {
+  if (!c || !O) return fail(OMVG_E_ARG, "null argument");
+  if (!(radius > 0.0)) return fail(OMVG_E_ARG, "radius must be > 0");
+  OMVG_CUDA(cudaSetDevice(c->device));
+  Plan p; int rc = plan_run(c, O, p); if (rc) return rc;
+  OMVG_CUDA(cudaMemcpyAsync(c->intr_mask.p, p.m.intr_mask.data(), c->ni * sizeof(unsigned), cudaMemcpyHostToDevice, c->stream));
+  OMVG_CUDA(cudaMemsetAsync(c->fail.p, 0, sizeof(int), c->stream));
+  bool have_scale = false; CoarseState coarse;
+  if ((rc = eval_jac(c, O, p.m, 0, have_scale)) || (rc = make_gauge(c, p)) || (rc = lm_diagonal(c, O, radius)) || (rc = assemble_reduced(c, p)) ||
+      (rc = refresh_coarse(c, p, coarse))) return rc;
+  const int nc6 = 6 * c->nc, nd = p.nd, np3 = 3 * c->np;
+  std::vector<double> hScc, hSci, hSii, hrhs(nd); std::vector<int> hrow, hcols;
+  if (S) {
+    hScc.resize(36 * (size_t)c->nnzb); hSci.resize((size_t)c->ni8 * nc6); hSii.resize((size_t)c->ni8 * c->ni8); hrow.resize(c->nc + 1); hcols.resize(c->nnzb);
+    OMVG_CUDA(cudaMemcpyAsync(hScc.data(), c->Scc.p, hScc.size() * 8, cudaMemcpyDeviceToHost, c->stream));
+    OMVG_CUDA(cudaMemcpyAsync(hSci.data(), c->Sci.p, hSci.size() * 8, cudaMemcpyDeviceToHost, c->stream));
+    OMVG_CUDA(cudaMemcpyAsync(hSii.data(), c->Sii.p, hSii.size() * 8, cudaMemcpyDeviceToHost, c->stream));
+    OMVG_CUDA(cudaMemcpyAsync(hrow.data(), c->rowptr.p, hrow.size() * 4, cudaMemcpyDeviceToHost, c->stream));
+    OMVG_CUDA(cudaMemcpyAsync(hcols.data(), c->cols.p, hcols.size() * 4, cudaMemcpyDeviceToHost, c->stream));
+  }
+  OMVG_CUDA(cudaMemcpyAsync(hrhs.data(), c->rhs.p, nd * 8, cudaMemcpyDeviceToHost, c->stream));
+  if ((rc = solve_reduced(c, O, p)) || (rc = back_substitute(c, p)) || (rc = read_scalars(c))) return rc;
+  std::vector<double> hz(nd), hstep(np3), hsc(np3 + nd), hlm(np3 + nd);
+  OMVG_CUDA(cudaMemcpyAsync(hz.data(), c->z.p, nd * 8, cudaMemcpyDeviceToHost, c->stream));
+  if (np3) OMVG_CUDA(cudaMemcpyAsync(hstep.data(), c->step_pt.p, np3 * 8, cudaMemcpyDeviceToHost, c->stream));
+  const double *sc_src[3] = {c->sc_pt.p, c->sc_cam.p, c->sc_intr.p}, *lm_src[3] = {c->lmD_pt.p, c->lmD_cam.p, c->lmD_intr.p};
+  const size_t off[4] = {0, (size_t)np3, (size_t)np3 + nc6, (size_t)np3 + nd};
+  for (int s = 0; s < 3; ++s) if (off[s + 1] > off[s]) {
+    OMVG_CUDA(cudaMemcpyAsync(hsc.data() + off[s], sc_src[s], (off[s + 1] - off[s]) * 8, cudaMemcpyDeviceToHost, c->stream));
+    OMVG_CUDA(cudaMemcpyAsync(hlm.data() + off[s], lm_src[s], (off[s + 1] - off[s]) * 8, cudaMemcpyDeviceToHost, c->stream));
+  }
+  OMVG_CUDA(cudaStreamSynchronize(c->stream));
+  int failflag; std::memcpy(&failflag, c->h_scal + S_COUNT + 192, sizeof(int));
+  if (failflag) { OMVG_CUDA(cudaMemsetAsync(c->fail.p, 0, sizeof(int), c->stream)); return fail(OMVG_E_NUMERIC, "reduced solve failed (code %d)", failflag); }
+  if (S) {
+    std::fill(S, S + (size_t)nd * nd, 0.0);
+    for (int a = 0; a < c->nc; ++a)                           // camera blocks (both triangles are stored)
+      for (int e = hrow[a]; e < hrow[a + 1]; ++e)
+        for (int k = 0; k < 36; ++k) S[(size_t)(6 * a + k / 6) * nd + 6 * hcols[e] + k % 6] = hScc[36 * (size_t)e + k];
+    for (int q = 0; q < c->ni8; ++q)                          // border Sci[q][camera column] and its transpose
+      for (int k = 0; k < nc6; ++k) { const double v = hSci[(size_t)q * nc6 + k]; S[(size_t)(nc6 + q) * nd + k] = v; S[(size_t)k * nd + nc6 + q] = v; }
+    for (int q = 0; q < c->ni8; ++q) for (int k = 0; k < c->ni8; ++k) S[(size_t)(nc6 + q) * nd + nc6 + k] = hSii[(size_t)q * c->ni8 + k];
+  }
+  if (scale) std::memcpy(scale, hsc.data(), hsc.size() * 8);
+  if (lm_diag) std::memcpy(lm_diag, hlm.data(), hlm.size() * 8);
+  if (rhs) std::memcpy(rhs, hrhs.data(), nd * 8);
+  if (z) std::memcpy(z, hz.data(), nd * 8);
+  if (step_point && np3) std::memcpy(step_point, hstep.data(), np3 * 8);
+  if (model_change) *model_change = c->h_scal[S_MODEL];
+  if (solver) *solver = (int32_t)p.solver;
+  if (pcg_stats) { pcg_stats[0] = c->h_scal[S_PCG_IT]; pcg_stats[1] = c->h_scal[S_PCG_RES]; pcg_stats[2] = c->h_scal[S_PCG_B]; }
+  return OMVG_OK;
+}
+
 }  // extern "C"
