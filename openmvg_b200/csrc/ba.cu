@@ -33,13 +33,6 @@ int model_nparams(int m) {     // size of the Ceres parameter block = getParams(
 }
 int model_ndata(int m) { return m == OMVG_CAMERA_SPHERICAL ? 2 : model_nparams(m); }   // doubles of the slot the kernels read
 
-template <typename T> struct DevBuf {
-  T *p = nullptr; size_t n = 0;
-  int alloc(size_t count) { release(); n = count; if (!count) return OMVG_OK; OMVG_CUDA(pool_malloc(reinterpret_cast<void **>(&p), count * sizeof(T))); return OMVG_OK; }
-  void release() { if (p) pool_free(p); p = nullptr; n = 0; }
-  ~DevBuf() { release(); }
-};
-
 }  // namespace
 
 // stream / events / pinned scalars of a context: creating and destroying them costs ~2.5 ms per Adjust, so
@@ -93,21 +86,8 @@ struct omvg_ba_ctx {
 
 namespace {
 
-// Every kernel of the context is launched through launch() or launch_coop() (grid-wide barriers), which check the launch
-// and count it: the run summary reports the count as kernel_launches.
-template <typename... P, typename... A>
-int launch(omvg_ba_ctx *c, void (*k)(P...), dim3 grid, dim3 block, size_t smem, A &&...args) {
-  k<<<grid, block, smem, c->stream>>>(std::forward<A>(args)...);
-  OMVG_CUDA(cudaGetLastError());
-  ++c->launches; return OMVG_OK;
-}
-template <typename T> struct NoDeduce { using type = T; };
-template <typename... P>
-int launch_coop(omvg_ba_ctx *c, void (*k)(P...), dim3 grid, dim3 block, size_t smem, typename NoDeduce<P>::type... args) {
-  void *argv[] = {&args...};
-  OMVG_CUDA(cudaLaunchCooperativeKernel((void *)k, grid, block, argv, smem, c->stream));
-  ++c->launches; return OMVG_OK;
-}
+// Every kernel of the context goes through launch() or launch_coop() (common.cuh): the run summary reports their count
+// as kernel_launches.
 
 // Calls f(std::integral_constant<int, K>{}) for the intrinsic columns in use (kiu = max getParams() size over the groups,
 // at least 3): the kernels that take KIU as a template parameter are instantiated for K = 3, 4, 6, 7 and 8 only.
@@ -741,13 +721,8 @@ int omvg_ba_create(omvg_ba_ctx **out, int device, const omvg_ba_problem *P) {
   PhaseTimer tm("create");
   int rc = validate(P); if (rc) return rc;
   tm.lap("validate");
-  int n = 0; OMVG_CUDA(cudaGetDeviceCount(&n));
-  if (device < 0 || device >= n) return fail(OMVG_E_CUDA, "no CUDA device %d (found %d)", device, n);
-  int cc_major = 0, cc_minor = 0, n_sms = 0;                 // attributes: cudaGetDeviceProperties costs milliseconds
-  OMVG_CUDA(cudaDeviceGetAttribute(&cc_major, cudaDevAttrComputeCapabilityMajor, device));
-  OMVG_CUDA(cudaDeviceGetAttribute(&cc_minor, cudaDevAttrComputeCapabilityMinor, device));
-  OMVG_CUDA(cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, device));
-  if (cc_major != 9 || cc_minor != 0) return fail(OMVG_E_CUDA, "device %d is sm_%d%d; this library is sm_90a only", device, cc_major, cc_minor);
+  int n_sms = 0;
+  if ((rc = check_device(device, &n_sms))) return rc;
   OMVG_CUDA(cudaSetDevice(device));
   omvg_ba_ctx *c = new omvg_ba_ctx; c->device = device; c->n_sms = n_sms;
   std::unique_ptr<omvg_ba_ctx, void (*)(omvg_ba_ctx *)> guard(c, [](omvg_ba_ctx *x) { omvg_ba_destroy(x); });

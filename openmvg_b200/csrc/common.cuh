@@ -1,4 +1,5 @@
-// common.cuh — error plumbing and the sm_90a PTX wrappers (mbarrier, TMA, wgmma) shared by match.cu and ba.cu.
+// common.cuh — error plumbing, owning buffers, checked launches, the device check and the sm_90a PTX wrappers (mbarrier,
+// TMA, wgmma) shared by match.cu, geom.cu and ba.cu.
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -8,6 +9,7 @@
 #include <map>
 #include <mutex>
 #include <unordered_map>
+#include <utility>
 
 #include "../../include/omvg_b200.h"
 
@@ -63,6 +65,56 @@ inline void pool_trim() {
   std::lock_guard<std::mutex> g(P.mu);
   for (int d = 0; d < 16; ++d) { for (auto &kv : P.free_[d]) cudaFree(kv.second); P.free_[d].clear(); }
   P.cached = 0;
+}
+
+// ----------------------------------------------------------------------------- owning buffers
+// Where a buffer's memory comes from: the caching pool above, the driver (cudaFree hands the memory back at once), or
+// pinned host memory.
+struct PoolAlloc { static cudaError_t get(void **p, size_t b) { return pool_malloc(p, b); } static void put(void *p) { pool_free(p); } };
+struct CudaAlloc { static cudaError_t get(void **p, size_t b) { return cudaMalloc(p, b); } static void put(void *p) { cudaFree(p); } };
+struct PinnedAlloc { static cudaError_t get(void **p, size_t b) { return cudaMallocHost(p, b); } static void put(void *p) { cudaFreeHost(p); } };
+
+// n elements of T, released when the buffer is destroyed or overwritten; movable, not copyable
+template <typename T, typename A = PoolAlloc> struct DevBuf {
+  T *p = nullptr; size_t n = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf &) = delete;
+  DevBuf &operator=(const DevBuf &) = delete;
+  DevBuf(DevBuf &&o) noexcept : p(o.p), n(o.n) { o.p = nullptr; o.n = 0; }
+  DevBuf &operator=(DevBuf &&o) noexcept { if (this != &o) { release(); std::swap(p, o.p); std::swap(n, o.n); } return *this; }
+  ~DevBuf() { release(); }
+  int alloc(size_t count) { release(); if (!count) return OMVG_OK; OMVG_CUDA(A::get(reinterpret_cast<void **>(&p), count * sizeof(T))); n = count; return OMVG_OK; }
+  int reserve(size_t count) { return count <= n ? OMVG_OK : alloc(count); }   // grow only; the old contents are lost
+  void release() { if (p) A::put(p); p = nullptr; n = 0; }
+};
+
+// ----------------------------------------------------------------------------- launches
+// Every kernel of a context (anything with a stream and a launch counter) is launched through launch() or launch_coop()
+// (grid-wide barriers), which check the launch and count it.
+template <typename C, typename... P, typename... A>
+int launch(C *c, void (*k)(P...), dim3 grid, dim3 block, size_t smem, A &&...args) {
+  k<<<grid, block, smem, c->stream>>>(std::forward<A>(args)...);
+  OMVG_CUDA(cudaGetLastError());
+  ++c->launches; return OMVG_OK;
+}
+template <typename T> struct NoDeduce { using type = T; };
+template <typename C, typename... P>
+int launch_coop(C *c, void (*k)(P...), dim3 grid, dim3 block, size_t smem, typename NoDeduce<P>::type... args) {
+  void *argv[] = {&args...};
+  OMVG_CUDA(cudaLaunchCooperativeKernel((void *)k, grid, block, argv, smem, c->stream));
+  ++c->launches; return OMVG_OK;
+}
+
+// the CUDA device exists and is an sm_90 part; its SM count out (attributes: cudaGetDeviceProperties costs milliseconds)
+inline int check_device(int device, int *n_sms) {
+  int n = 0; OMVG_CUDA(cudaGetDeviceCount(&n));
+  if (device < 0 || device >= n) return fail(OMVG_E_CUDA, "no CUDA device %d (found %d)", device, n);
+  int cc_major = 0, cc_minor = 0;
+  OMVG_CUDA(cudaDeviceGetAttribute(&cc_major, cudaDevAttrComputeCapabilityMajor, device));
+  OMVG_CUDA(cudaDeviceGetAttribute(&cc_minor, cudaDevAttrComputeCapabilityMinor, device));
+  OMVG_CUDA(cudaDeviceGetAttribute(n_sms, cudaDevAttrMultiProcessorCount, device));
+  if (cc_major != 9 || cc_minor != 0) return fail(OMVG_E_CUDA, "device %d is sm_%d%d; this library is sm_90a only", device, cc_major, cc_minor);
+  return OMVG_OK;
 }
 
 // ----------------------------------------------------------------------------- mbarrier

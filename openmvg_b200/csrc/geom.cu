@@ -753,19 +753,6 @@ __global__ void __launch_bounds__(THREADS) acransac_kernel(Args A) {
 
 namespace {
 
-// the CUDA device exists and is an sm_90 part; its SM count out
-int check_device(int device, int *n_sms) {
-  using namespace omvg;
-  int n = 0; OMVG_CUDA(cudaGetDeviceCount(&n));
-  if (device < 0 || device >= n) return fail(OMVG_E_CUDA, "no CUDA device %d (found %d)", device, n);
-  int cc_major = 0, cc_minor = 0;
-  OMVG_CUDA(cudaDeviceGetAttribute(&cc_major, cudaDevAttrComputeCapabilityMajor, device));
-  OMVG_CUDA(cudaDeviceGetAttribute(&cc_minor, cudaDevAttrComputeCapabilityMinor, device));
-  OMVG_CUDA(cudaDeviceGetAttribute(n_sms, cudaDevAttrMultiProcessorCount, device));
-  if (cc_major != 9 || cc_minor != 0) return fail(OMVG_E_CUDA, "device %d is sm_%d%d; this library is sm_90a only", device, cc_major, cc_minor);
-  return OMVG_OK;
-}
-
 // everything after the per-model argument checks; intr (model OMVG_GEOM_ESSENTIAL only): [n_pairs][6]
 int geom_run(int device, int32_t model, uint64_t n_pairs, const uint64_t *offsets, const double *xI, const double *xJ,
              const int32_t *image_size, const double *intr, double precision, uint32_t max_iterations,
@@ -787,35 +774,35 @@ int geom_run(int device, int32_t model, uint64_t n_pairs, const uint64_t *offset
   const bool essential = model == OMVG_GEOM_ESSENTIAL;
   const size_t xs = essential ? 24 : 16;                  // scratch per match: bearing vectors (E) or normalised points
   OMVG_CUDA(cudaSetDevice(device));
-  cudaStream_t st; OMVG_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-  struct Bufs { std::vector<void *> p; cudaStream_t s; ~Bufs() { for (void *q : p) pool_free(q); cudaStreamDestroy(s); } } B{{}, st};
-  auto dalloc = [&](size_t bytes) -> void * { void *q = nullptr; if (pool_malloc(&q, std::max<size_t>(bytes, 8)) != cudaSuccess) return nullptr; B.p.push_back(q); return q; };
+  struct Call { cudaStream_t stream = nullptr; long long launches = 0; ~Call() { if (stream) cudaStreamDestroy(stream); } } call;
+  OMVG_CUDA(cudaStreamCreateWithFlags(&call.stream, cudaStreamNonBlocking));
+  const cudaStream_t st = call.stream;
+  const size_t m1 = std::max<uint64_t>(nm, 1);            // no buffer is empty
+  DevBuf<unsigned long long> d_off; DevBuf<double> d_xI, d_xJ, d_x1, d_x2, d_F, d_stats, d_intr; DevBuf<int> d_sz;
+  DevBuf<float> d_ln, d_lk, d_l10; DevBuf<uint32_t> d_idx, d_inl, d_ninl;
+  if (d_off.alloc(n_pairs + 1) || d_xI.alloc(2 * m1) || d_xJ.alloc(2 * m1) || d_x1.alloc(xs / 8 * m1) || d_x2.alloc(xs / 8 * m1) ||
+      d_sz.alloc(4 * n_pairs) || d_ln.alloc(nm + n_pairs) || d_lk.alloc(nm + n_pairs) || d_l10.alloc(nm + n_pairs) ||
+      d_idx.alloc(m1) || d_inl.alloc(m1) || d_ninl.alloc(n_pairs) || d_F.alloc(9 * n_pairs) || d_stats.alloc(2 * n_pairs) ||
+      (essential && d_intr.alloc(6 * n_pairs)))
+    return fail(OMVG_E_CUDA, "out of device memory");
+  if (essential) OMVG_CUDA(cudaMemcpyAsync(d_intr.p, intr, n_pairs * 48, cudaMemcpyHostToDevice, st));
+  OMVG_CUDA(cudaMemcpyAsync(d_off.p, offsets, (n_pairs + 1) * 8, cudaMemcpyHostToDevice, st));
+  OMVG_CUDA(cudaMemcpyAsync(d_sz.p, image_size, n_pairs * 16, cudaMemcpyHostToDevice, st));
+  if (nm) { OMVG_CUDA(cudaMemcpyAsync(d_xI.p, xI, nm * 16, cudaMemcpyHostToDevice, st)); OMVG_CUDA(cudaMemcpyAsync(d_xJ.p, xJ, nm * 16, cudaMemcpyHostToDevice, st)); }
   geom::Args A{};
-  unsigned long long *d_off = (unsigned long long *)dalloc((n_pairs + 1) * 8);
-  double *d_xI = (double *)dalloc(nm * 16), *d_xJ = (double *)dalloc(nm * 16), *d_x1 = (double *)dalloc(nm * xs), *d_x2 = (double *)dalloc(nm * xs);
-  int *d_sz = (int *)dalloc(n_pairs * 16);
-  float *d_ln = (float *)dalloc((nm + n_pairs) * 4), *d_lk = (float *)dalloc((nm + n_pairs) * 4), *d_l10 = (float *)dalloc((nm + n_pairs) * 4);
-  uint32_t *d_idx = (uint32_t *)dalloc(nm * 4), *d_inl = (uint32_t *)dalloc(nm * 4), *d_ninl = (uint32_t *)dalloc(n_pairs * 4);
-  double *d_F = (double *)dalloc(n_pairs * 72), *d_stats = (double *)dalloc(n_pairs * 16);
-  double *d_intr = essential ? (double *)dalloc(n_pairs * 48) : nullptr;
-  if (!d_off || !d_xI || !d_xJ || !d_x1 || !d_x2 || !d_sz || !d_ln || !d_lk || !d_l10 || !d_idx || !d_inl || !d_ninl || !d_F || !d_stats || (essential && !d_intr)) return fail(OMVG_E_CUDA, "out of device memory");
-  if (essential) OMVG_CUDA(cudaMemcpyAsync(d_intr, intr, n_pairs * 48, cudaMemcpyHostToDevice, st));
-  OMVG_CUDA(cudaMemcpyAsync(d_off, offsets, (n_pairs + 1) * 8, cudaMemcpyHostToDevice, st));
-  OMVG_CUDA(cudaMemcpyAsync(d_sz, image_size, n_pairs * 16, cudaMemcpyHostToDevice, st));
-  if (nm) { OMVG_CUDA(cudaMemcpyAsync(d_xI, xI, nm * 16, cudaMemcpyHostToDevice, st)); OMVG_CUDA(cudaMemcpyAsync(d_xJ, xJ, nm * 16, cudaMemcpyHostToDevice, st)); }
   A.model = model;
-  A.offsets = d_off; A.xI = d_xI; A.xJ = d_xJ; A.image_size = d_sz; A.precision = precision; A.iterations = max_iterations;
-  A.x1 = d_x1; A.x2 = d_x2; A.logc_n = d_ln; A.logc_k = d_lk; A.l10 = d_l10; A.vec_index = d_idx; A.inliers = d_inl; A.n_inliers = d_ninl; A.F = d_F; A.stats = d_stats;
-  A.n_pairs = (unsigned int)n_pairs; A.intr = d_intr;
+  A.offsets = d_off.p; A.xI = d_xI.p; A.xJ = d_xJ.p; A.image_size = d_sz.p; A.precision = precision; A.iterations = max_iterations;
+  A.x1 = d_x1.p; A.x2 = d_x2.p; A.logc_n = d_ln.p; A.logc_k = d_lk.p; A.l10 = d_l10.p; A.vec_index = d_idx.p; A.inliers = d_inl.p;
+  A.n_inliers = d_ninl.p; A.F = d_F.p; A.stats = d_stats.p;
+  A.n_pairs = (unsigned int)n_pairs; A.intr = d_intr.p;
   void (*kernel)(geom::Args) = essential ? geom::acransac_kernel<true> : geom::acransac_kernel<false>;
   int per_sm = 1; OMVG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, geom::THREADS, 0));
   const unsigned int grid = (unsigned int)std::min<uint64_t>(n_pairs, (uint64_t)n_sms * std::max(1, per_sm));
-  kernel<<<grid, geom::THREADS, 0, st>>>(A);
-  OMVG_CUDA(cudaGetLastError());
-  if (nm) OMVG_CUDA(cudaMemcpyAsync(inliers, d_inl, nm * 4, cudaMemcpyDeviceToHost, st));
-  OMVG_CUDA(cudaMemcpyAsync(n_inliers, d_ninl, n_pairs * 4, cudaMemcpyDeviceToHost, st));
-  OMVG_CUDA(cudaMemcpyAsync(F, d_F, n_pairs * 72, cudaMemcpyDeviceToHost, st));
-  OMVG_CUDA(cudaMemcpyAsync(stats, d_stats, n_pairs * 16, cudaMemcpyDeviceToHost, st));
+  if (const int rc = launch(&call, kernel, grid, geom::THREADS, 0, A)) return rc;
+  if (nm) OMVG_CUDA(cudaMemcpyAsync(inliers, d_inl.p, nm * 4, cudaMemcpyDeviceToHost, st));
+  OMVG_CUDA(cudaMemcpyAsync(n_inliers, d_ninl.p, n_pairs * 4, cudaMemcpyDeviceToHost, st));
+  OMVG_CUDA(cudaMemcpyAsync(F, d_F.p, n_pairs * 72, cudaMemcpyDeviceToHost, st));
+  OMVG_CUDA(cudaMemcpyAsync(stats, d_stats.p, n_pairs * 16, cudaMemcpyDeviceToHost, st));
   OMVG_CUDA(cudaStreamSynchronize(st));
   return OMVG_OK;
 }
@@ -850,14 +837,13 @@ extern "C" int omvg_geom_debug_five_point(int device, uint32_t n, const double *
   if (const int rc = check_device(device, &n_sms)) return rc;
   if (!n) return OMVG_OK;
   OMVG_CUDA(cudaSetDevice(device));
-  double *d_b1 = nullptr, *d_b2 = nullptr, *d_E = nullptr; int *d_n = nullptr;
-  struct Bufs { void **p[4]; ~Bufs() { for (void **q : p) if (*q) cudaFree(*q); } } B{{(void **)&d_b1, (void **)&d_b2, (void **)&d_E, (void **)&d_n}};
-  OMVG_CUDA(cudaMalloc(&d_b1, n * 120ull)); OMVG_CUDA(cudaMalloc(&d_b2, n * 120ull));
-  OMVG_CUDA(cudaMalloc(&d_E, n * 720ull)); OMVG_CUDA(cudaMalloc(&d_n, n * 4ull));
-  OMVG_CUDA(cudaMemcpy(d_b1, b1, n * 120ull, cudaMemcpyHostToDevice)); OMVG_CUDA(cudaMemcpy(d_b2, b2, n * 120ull, cudaMemcpyHostToDevice));
-  geom::five_point_kernel<<<std::min<uint32_t>(n, 64u * n_sms), 32>>>(n, d_b1, d_b2, d_E, d_n);
+  DevBuf<double, CudaAlloc> d_b1, d_b2, d_E; DevBuf<int, CudaAlloc> d_n;
+  int rc;
+  if ((rc = d_b1.alloc(15ull * n)) || (rc = d_b2.alloc(15ull * n)) || (rc = d_E.alloc(90ull * n)) || (rc = d_n.alloc(n))) return rc;
+  OMVG_CUDA(cudaMemcpy(d_b1.p, b1, n * 120ull, cudaMemcpyHostToDevice)); OMVG_CUDA(cudaMemcpy(d_b2.p, b2, n * 120ull, cudaMemcpyHostToDevice));
+  geom::five_point_kernel<<<std::min<uint32_t>(n, 64u * n_sms), 32>>>(n, d_b1.p, d_b2.p, d_E.p, d_n.p);
   OMVG_CUDA(cudaGetLastError());
-  OMVG_CUDA(cudaMemcpy(E, d_E, n * 720ull, cudaMemcpyDeviceToHost)); OMVG_CUDA(cudaMemcpy(n_models, d_n, n * 4ull, cudaMemcpyDeviceToHost));
+  OMVG_CUDA(cudaMemcpy(E, d_E.p, n * 720ull, cudaMemcpyDeviceToHost)); OMVG_CUDA(cudaMemcpy(n_models, d_n.p, n * 4ull, cudaMemcpyDeviceToHost));
   return OMVG_OK;
 }
 

@@ -28,6 +28,7 @@
 #include <cmath>
 #include <climits>
 #include <cstring>
+#include <memory>
 #include <vector>
 
 namespace omvg {
@@ -838,36 +839,46 @@ __global__ void __launch_bounds__(FIN_THREADS) guided_compact_kernel(const PairI
 // ===================================================================================== host side
 using namespace omvg;
 
+namespace omvg {
+template <typename T> using Buf = DevBuf<T, CudaAlloc>;   // the arena goes back to the driver with its image set
+
+// everything tied to one image set (omvg_match_set_images): dropping it is a reset
+struct ImageSet {
+  uint32_t n_images = 0, total_rows = 0;
+  std::vector<uint32_t> counts, row0, group;
+  Buf<uint8_t> d_desc; Buf<int32_t> d_norm, d_ckey;
+  Buf<uint32_t> d_img_row0, d_img_count, d_img_group, d_row_img;
+  bool prepared = false;
+  CUtensorMap tmap, tmap_dig;
+  // fifth-slice kernel (match_wgmma_kernel<true>): 32 signed digits per arena row, per-image offset c0, eligibility
+  Buf<uint4> d_dig; Buf<int32_t> d_img_c0; Buf<int2> d_hmm; std::vector<int32_t> c0; bool use_dig = false;
+  // cascade hashing state (omvg_match_cascade_prepare)
+  Buf<uint4> d_code, d_bid; Buf<uint32_t> d_bstart, d_bitems; Buf<float> d_proj, d_zm;
+  bool cascade_ready = false; std::vector<float> h_zm;
+  // guided matching (omvg_match_upload_positions / omvg_match_guided_run): one double2 per arena row
+  Buf<double2> d_pos; std::vector<uint8_t> has_pos;
+  bool loaded() const { return d_desc.p != nullptr; }
+};
+}  // namespace omvg
+
 struct omvg_match_ctx {
   int device = 0, n_sms = 0;
   cudaStream_t stream = nullptr;
-  uint32_t n_images = 0, total_rows = 0;
-  std::vector<uint32_t> counts, row0, group;
-  uint8_t *d_desc = nullptr; int32_t *d_norm = nullptr, *d_ckey = nullptr;
-  uint32_t *d_img_row0 = nullptr, *d_img_count = nullptr, *d_img_group = nullptr, *d_row_img = nullptr;
-  bool uploaded = false, prepared = false;
-  CUtensorMap tmap, tmap_dig;
-  // fifth-slice kernel (match_wgmma_kernel<true>): 32 signed digits per arena row, per-image offset c0, eligibility
-  uint4 *d_dig = nullptr; int32_t *d_img_c0 = nullptr; int2 *d_hmm = nullptr; std::vector<int32_t> c0; bool use_dig = false;
+  ImageSet img;
   // run state
-  int2 *d_k12 = nullptr; size_t k12_cap = 0;           // in int2 elements
-  Unit *d_units = nullptr; size_t units_cap = 0;
-  PairInfo *d_pairs = nullptr; uint32_t *d_counts = nullptr; size_t pairs_cap = 0;
-  uint64_t *d_offsets = nullptr; size_t offsets_cap = 0;   // n_pairs + 1 (global)
-  uint64_t *d_total = nullptr;
-  uint2 *d_out = nullptr; size_t out_cap = 0;
+  Buf<int2> d_k12;
+  Buf<Unit> d_units;
+  Buf<PairInfo> d_pairs; Buf<uint32_t> d_counts;
+  Buf<uint64_t> d_offsets;   // n_pairs + 1 (global)
+  Buf<uint64_t> d_total;
+  Buf<uint2> d_out;
+  Buf<GuidedModel> d_models;
   uint64_t n_pairs_last = 0, total_last = 0; bool have_result = false;
-  uint64_t *h_offsets = nullptr; size_t h_offsets_cap = 0; uint32_t *h_ij = nullptr; size_t h_ij_cap = 0;
+  DevBuf<uint64_t, PinnedAlloc> h_offsets; DevBuf<uint2, PinnedAlloc> h_ij;
   uint64_t launches = 0;
   double tc_ms = 0; uint64_t tc_launches = 0; std::vector<std::pair<cudaEvent_t, cudaEvent_t>> pending;
   std::vector<cudaEvent_t> ev_pool;
   size_t k12_budget_bytes = size_t(2) << 30;
-  // cascade hashing state (omvg_match_cascade_prepare)
-  uint4 *d_code = nullptr, *d_bid = nullptr; uint32_t *d_bstart = nullptr, *d_bitems = nullptr; float *d_proj = nullptr, *d_zm = nullptr;
-  bool cascade_ready = false; std::vector<float> h_zm;
-  // guided matching (omvg_match_upload_positions / omvg_match_guided_run): one double2 per arena row
-  double2 *d_pos = nullptr; std::vector<uint8_t> has_pos;
-  GuidedModel *d_models = nullptr; size_t models_cap = 0;
 };
 
 namespace {
@@ -876,44 +887,26 @@ typedef CUresult (*encode_tiled_fn)(CUtensorMap *, CUtensorMapDataType, cuuint32
                                     const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-int make_tmap(omvg_match_ctx *c) {
+int make_tmap(ImageSet &s) {
   void *fn = nullptr; cudaDriverEntryPointQueryResult qres;
   OMVG_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
   if (!fn || qres != cudaDriverEntryPointSuccess) return fail(OMVG_E_CUDA, "cuTensorMapEncodeTiled not available");
-  const cuuint64_t dims[2] = {OMVG_DESC_LEN, c->total_rows};
+  const cuuint64_t dims[2] = {OMVG_DESC_LEN, s.total_rows};
   const cuuint64_t strides[1] = {OMVG_DESC_LEN};
   const cuuint32_t box[2] = {OMVG_DESC_LEN, 128};
   const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = ((encode_tiled_fn)fn)(&c->tmap, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, c->d_desc, dims, strides, box, estr,
+  const CUresult r = ((encode_tiled_fn)fn)(&s.tmap, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, s.d_desc.p, dims, strides, box, estr,
                                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(OMVG_E_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)r);
-  const cuuint64_t ddims[2] = {DIG_LEN, c->total_rows};
+  const cuuint64_t ddims[2] = {DIG_LEN, s.total_rows};
   const cuuint64_t dstrides[1] = {DIG_LEN};
   const cuuint32_t dbox[2] = {DIG_LEN, TILE_DB};
-  const CUresult r2 = ((encode_tiled_fn)fn)(&c->tmap_dig, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, c->d_dig, ddims, dstrides, dbox, estr,
+  const CUresult r2 = ((encode_tiled_fn)fn)(&s.tmap_dig, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, s.d_dig.p, ddims, dstrides, dbox, estr,
                                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_32B,
                                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r2 != CUDA_SUCCESS) return fail(OMVG_E_CUDA, "cuTensorMapEncodeTiled (digits) failed (%d)", (int)r2);
   return OMVG_OK;
-}
-
-void free_images(omvg_match_ctx *c) {
-  cudaFree(c->d_code); cudaFree(c->d_bid); cudaFree(c->d_bstart); cudaFree(c->d_bitems); cudaFree(c->d_proj); cudaFree(c->d_zm);
-  c->d_code = c->d_bid = nullptr; c->d_bstart = c->d_bitems = nullptr; c->d_proj = c->d_zm = nullptr; c->cascade_ready = false;
-  cudaFree(c->d_desc); cudaFree(c->d_norm); cudaFree(c->d_ckey); cudaFree(c->d_img_row0); cudaFree(c->d_img_count);
-  cudaFree(c->d_img_group); cudaFree(c->d_row_img); cudaFree(c->d_dig); cudaFree(c->d_img_c0); cudaFree(c->d_hmm);
-  c->d_dig = nullptr; c->d_img_c0 = nullptr; c->d_hmm = nullptr; c->use_dig = false;
-  c->d_desc = nullptr; c->d_norm = c->d_ckey = nullptr; c->d_img_row0 = c->d_img_count = c->d_img_group = c->d_row_img = nullptr;
-  cudaFree(c->d_pos); c->d_pos = nullptr; c->has_pos.clear();
-}
-
-template <typename T> int ensure(T *&p, size_t &cap, size_t need) {
-  if (need <= cap) return OMVG_OK;
-  if (p) cudaFree(p);
-  p = nullptr; cap = 0;
-  OMVG_CUDA(cudaMalloc(&p, need * sizeof(T)));
-  cap = need; return OMVG_OK;
 }
 
 int drain_timers(omvg_match_ctx *c) {
@@ -928,24 +921,21 @@ cudaEvent_t get_event(omvg_match_ctx *c) {
   cudaEvent_t e; cudaEventCreate(&e); return e;
 }
 
-// per-pair device table of one batch (d_pairs / d_counts), grown on demand
-int ensure_pairs(omvg_match_ctx *c, uint32_t nb) {
-  if (nb <= c->pairs_cap) return OMVG_OK;
-  if (c->d_pairs) cudaFree(c->d_pairs); if (c->d_counts) cudaFree(c->d_counts);
-  c->d_pairs = nullptr; c->d_counts = nullptr; c->pairs_cap = 0;
-  OMVG_CUDA(cudaMalloc(&c->d_pairs, nb * sizeof(PairInfo))); OMVG_CUDA(cudaMalloc(&c->d_counts, nb * sizeof(uint32_t)));
-  c->pairs_cap = nb; return OMVG_OK;
+// a matcher kernel between two events: omvg_match_kernel_time reports the sum of these intervals
+template <typename... P, typename... A>
+int timed_launch(omvg_match_ctx *c, void (*k)(P...), dim3 grid, dim3 block, size_t smem, A &&...args) {
+  const cudaEvent_t e0 = get_event(c), e1 = get_event(c);
+  OMVG_CUDA(cudaEventRecord(e0, c->stream));
+  if (const int rc = launch(c, k, grid, block, smem, std::forward<A>(args)...)) return rc;
+  OMVG_CUDA(cudaEventRecord(e1, c->stream));
+  c->pending.emplace_back(e0, e1); c->tc_launches++; return OMVG_OK;
 }
 
 // a new CSR result over n_pairs pairs: offsets[0] = 0, running total 0
 int begin_result(omvg_match_ctx *c, uint64_t n_pairs) {
-  if (n_pairs + 1 > c->offsets_cap) {
-    if (c->d_offsets) cudaFree(c->d_offsets);
-    c->d_offsets = nullptr; c->offsets_cap = 0;
-    OMVG_CUDA(cudaMalloc(&c->d_offsets, (n_pairs + 1) * sizeof(uint64_t))); c->offsets_cap = n_pairs + 1;
-  }
-  OMVG_CUDA(cudaMemsetAsync(c->d_total, 0, sizeof(uint64_t), c->stream));
-  OMVG_CUDA(cudaMemsetAsync(c->d_offsets, 0, sizeof(uint64_t), c->stream));
+  if (const int rc = c->d_offsets.reserve(n_pairs + 1)) return rc;
+  OMVG_CUDA(cudaMemsetAsync(c->d_total.p, 0, sizeof(uint64_t), c->stream));
+  OMVG_CUDA(cudaMemsetAsync(c->d_offsets.p, 0, sizeof(uint64_t), c->stream));
   c->total_last = 0; c->n_pairs_last = n_pairs; c->have_result = false;
   return OMVG_OK;
 }
@@ -953,69 +943,70 @@ int begin_result(omvg_match_ctx *c, uint64_t n_pairs) {
 // the per-pair counts of batch [p0, p0 + nb) are in d_counts and each pair's rows sit compacted at the start of its
 // d_k12 segment: scan the counts into the global offsets and append the rows to d_out
 int gather_batch(omvg_match_ctx *c, uint32_t nb, uint64_t p0) {
-  scan_counts_kernel<<<1, 1024, 0, c->stream>>>(c->d_counts, nb, c->d_offsets + p0, c->d_total);
-  OMVG_CUDA(cudaGetLastError());
-  c->launches++;
+  int rc;
+  if ((rc = launch(c, scan_counts_kernel, 1, 1024, 0, c->d_counts.p, nb, c->d_offsets.p + p0, c->d_total.p))) return rc;
   // size the global output buffer: needs the running total (one small sync per batch)
   uint64_t total = 0;
-  OMVG_CUDA(cudaMemcpyAsync(&total, c->d_total, sizeof total, cudaMemcpyDeviceToHost, c->stream));
+  OMVG_CUDA(cudaMemcpyAsync(&total, c->d_total.p, sizeof total, cudaMemcpyDeviceToHost, c->stream));
   OMVG_CUDA(cudaStreamSynchronize(c->stream));
-  if (total > c->out_cap) {
-    const size_t ncap = std::max<size_t>(total, c->out_cap * 2 + 1024);
-    uint2 *n = nullptr; OMVG_CUDA(cudaMalloc(&n, ncap * sizeof(uint2)));
-    if (c->d_out && c->total_last) OMVG_CUDA(cudaMemcpyAsync(n, c->d_out, c->total_last * sizeof(uint2), cudaMemcpyDeviceToDevice, c->stream));
+  if (total > c->d_out.n) {
+    Buf<uint2> n;
+    if ((rc = n.alloc(std::max<size_t>(total, c->d_out.n * 2 + 1024)))) return rc;
+    if (c->d_out.p && c->total_last) OMVG_CUDA(cudaMemcpyAsync(n.p, c->d_out.p, c->total_last * sizeof(uint2), cudaMemcpyDeviceToDevice, c->stream));
     OMVG_CUDA(cudaStreamSynchronize(c->stream));
-    if (c->d_out) cudaFree(c->d_out);
-    c->d_out = n; c->out_cap = ncap;
+    c->d_out = std::move(n);
   }
-  compact_kernel<<<nb, 128, 0, c->stream>>>(c->d_k12, c->d_pairs, c->d_counts, c->d_offsets + p0, c->d_out);
-  OMVG_CUDA(cudaGetLastError());
-  c->launches++;
+  if ((rc = launch(c, compact_kernel, nb, 128, 0, c->d_k12.p, c->d_pairs.p, c->d_counts.p, c->d_offsets.p + p0, c->d_out.p))) return rc;
   c->total_last = total;
   return OMVG_OK;
 }
 
-// one batch of pairs: tensor-core kernel + finalize + scan + compact
-int run_batch(omvg_match_ctx *c, const uint32_t *pi, const uint32_t *pj, uint64_t p0, uint64_t p1, float fratio,
-              std::vector<Unit> &units, std::vector<PairInfo> &pinfo) {
-  units.clear(); pinfo.clear();
-  size_t out = 0, n_units = 0;
-  for (uint64_t p = p0; p < p1; ++p) {
-    const uint32_t I = pi[p], J = pj[p];
-    PairInfo P{}; P.db_row0 = c->row0[I]; P.db_count = c->counts[I]; P.db_group = c->group[I]; P.db_c0 = c->c0.empty() ? 0 : c->c0[I];
-    P.q_row0 = c->row0[J]; P.q_count = c->counts[J]; P.out_off = out;
-    // Matcher_Regions.cpp:65-69,85-90 (empty regions) and matcher_brute_force.hpp:108-113 (NN > rows)
-    const bool active = P.db_count >= 2 && P.q_count >= 1;
-    if (!active) P.q_count = 0;
-    pinfo.push_back(P);
-    if (!active) continue;
-    const uint32_t qt = (P.q_count + TILE_Q - 1) / TILE_Q;
-    pinfo.back().unit0 = (uint32_t)n_units; n_units += qt;
-    out += size_t(qt) * TILE_Q;
-  }
-  if (out > 0xffffffffull) return fail(OMVG_E_ARG, "batch too large");
-  const uint32_t nb = (uint32_t)(p1 - p0);
+// What a pair costs the d_k12 budget (int2 rows): it joins a batch that has used `used` while used + need fits the
+// budget, and the batch has then used used + use.
+struct Cost { size_t need, use; };
+
+// The pair loop of omvg_match_run, _cascade_run and _guided_run.  The pairs are cut into batches of at most `cap` pairs
+// within the d_k12 budget (a batch takes at least one pair).  fill(p, P) fills the PairInfo of pair p, whose out_off is
+// set, and returns the d_k12 rows it takes.  launches(p0, nb, rows, max q_count) runs the path's kernels on the
+// uploaded table of batch [p0, p0 + nb): they leave the per-pair counts in d_counts and each pair's rows compacted at
+// the start of its d_k12 segment.
+template <typename CostF, typename FillF, typename LaunchF>
+int run_pairs(omvg_match_ctx *c, const uint32_t *pair_i, const uint32_t *pair_j, uint64_t n_pairs, uint64_t cap,
+              CostF cost, FillF fill, LaunchF launches) {
+  for (uint64_t p = 0; p < n_pairs; ++p)
+    if (pair_i[p] >= c->img.n_images || pair_j[p] >= c->img.n_images) return fail(OMVG_E_ARG, "pair %llu out of range", (unsigned long long)p);
   int rc;
-  if ((rc = ensure(c->d_k12, c->k12_cap, std::max<size_t>(out, 1)))) return rc;
-  if ((rc = ensure(c->d_units, c->units_cap, std::max<size_t>(n_units, 1)))) return rc;
-  if ((rc = ensure_pairs(c, nb))) return rc;
-  OMVG_CUDA(cudaMemcpyAsync(c->d_pairs, pinfo.data(), nb * sizeof(PairInfo), cudaMemcpyHostToDevice, c->stream));
-  if (n_units) {
-    expand_units_kernel<<<nb, 64, 0, c->stream>>>(c->d_pairs, c->d_units); OMVG_CUDA(cudaGetLastError()); c->launches++;
-    const uint32_t grid = (uint32_t)std::min<size_t>(n_units, (size_t)c->n_sms);
-    cudaEvent_t e0 = get_event(c), e1 = get_event(c);
-    OMVG_CUDA(cudaEventRecord(e0, c->stream));
-    if (c->use_dig) match_wgmma_kernel<true><<<grid, MATCH_THREADS, match_smem_bytes<true>(), c->stream>>>(c->tmap, c->tmap_dig, c->d_ckey, c->d_units, (uint32_t)n_units, c->d_k12);
-    else match_wgmma_kernel<false><<<grid, MATCH_THREADS, match_smem_bytes<false>(), c->stream>>>(c->tmap, c->tmap_dig, c->d_ckey, c->d_units, (uint32_t)n_units, c->d_k12);
-    OMVG_CUDA(cudaGetLastError());
-    OMVG_CUDA(cudaEventRecord(e1, c->stream));
-    c->pending.emplace_back(e0, e1); c->tc_launches++; c->launches++;
+  if ((rc = begin_result(c, n_pairs))) return rc;
+  const size_t budget = c->k12_budget_bytes / sizeof(int2);
+  std::vector<PairInfo> pinfo;
+  for (uint64_t p0 = 0, p1; p0 < n_pairs; p0 = p1) {
+    pinfo.clear(); size_t used = 0, rows = 0; uint32_t maxq = 0;
+    for (p1 = p0; p1 < n_pairs && p1 - p0 < cap; ++p1) {
+      const Cost k = cost(p1);
+      if (p1 > p0 && used + k.need > budget) break;
+      used += k.use;
+      PairInfo P{}; P.out_off = rows; rows += fill(p1, P);
+      maxq = std::max(maxq, P.q_count); pinfo.push_back(P);
+    }
+    if (rows > 0xffffffffull) return fail(OMVG_E_ARG, "batch too large");
+    const uint32_t nb = (uint32_t)(p1 - p0);
+    if ((rc = c->d_k12.reserve(std::max<size_t>(rows, 1))) || (rc = c->d_pairs.reserve(nb)) || (rc = c->d_counts.reserve(nb))) return rc;
+    OMVG_CUDA(cudaMemcpyAsync(c->d_pairs.p, pinfo.data(), nb * sizeof(PairInfo), cudaMemcpyHostToDevice, c->stream));
+    if ((rc = launches(p0, nb, rows, maxq)) || (rc = gather_batch(c, nb, p0))) return rc;
   }
-  if (c->use_dig) match_finalize_kernel<true><<<nb, FIN_THREADS, 0, c->stream>>>(c->d_desc, c->d_norm, c->d_pairs, c->d_k12, c->d_counts, fratio);
-  else match_finalize_kernel<false><<<nb, FIN_THREADS, 0, c->stream>>>(c->d_desc, c->d_norm, c->d_pairs, c->d_k12, c->d_counts, fratio);
-  OMVG_CUDA(cudaGetLastError());
-  c->launches++;
-  return gather_batch(c, nb, p0);
+  c->have_result = true; return OMVG_OK;
+}
+
+// one image's descriptors into the arena
+int upload_desc(omvg_match_ctx *c, uint32_t image, const void *desc, cudaMemcpyKind kind) {
+  if (!c) return fail(OMVG_E_ARG, "bad image %u", image);
+  ImageSet &im = c->img;
+  if (!im.loaded()) return fail(OMVG_E_STATE, "set_images first");
+  if (image >= im.n_images || (!desc && im.counts[image])) return fail(OMVG_E_ARG, "bad image %u", image);
+  OMVG_CUDA(cudaSetDevice(c->device));
+  if (im.counts[image])
+    OMVG_CUDA(cudaMemcpyAsync(im.d_desc.p + (size_t)im.row0[image] * OMVG_DESC_LEN, desc, (size_t)im.counts[image] * OMVG_DESC_LEN, kind, c->stream));
+  im.prepared = false; im.cascade_ready = false; return OMVG_OK;
 }
 
 }  // namespace
@@ -1032,156 +1023,155 @@ int omvg_device_count(void) {
 
 int omvg_match_create(omvg_match_ctx **out, int device) {
   if (!out) return fail(OMVG_E_ARG, "null ctx");
-  int n = 0; OMVG_CUDA(cudaGetDeviceCount(&n));
-  if (device < 0 || device >= n) return fail(OMVG_E_CUDA, "no CUDA device %d (found %d)", device, n);
-  int cc_major = 0, cc_minor = 0, n_sms = 0;
-  OMVG_CUDA(cudaDeviceGetAttribute(&cc_major, cudaDevAttrComputeCapabilityMajor, device));
-  OMVG_CUDA(cudaDeviceGetAttribute(&cc_minor, cudaDevAttrComputeCapabilityMinor, device));
-  OMVG_CUDA(cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, device));
-  if (cc_major != 9 || cc_minor != 0) return fail(OMVG_E_CUDA, "device %d is sm_%d%d; this library is sm_90a only", device, cc_major, cc_minor);
+  int n_sms = 0;
+  if (const int rc = check_device(device, &n_sms)) return rc;
   OMVG_CUDA(cudaSetDevice(device));
-  omvg_match_ctx *c = new omvg_match_ctx; c->device = device; c->n_sms = n_sms;
+  std::unique_ptr<omvg_match_ctx, int (*)(omvg_match_ctx *)> c(new omvg_match_ctx, omvg_match_destroy);
+  c->device = device; c->n_sms = n_sms;
   OMVG_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
   OMVG_CUDA(cudaFuncSetAttribute(match_wgmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, match_smem_bytes<false>()));
   OMVG_CUDA(cudaFuncSetAttribute(match_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, match_smem_bytes<true>()));
-  OMVG_CUDA(cudaMalloc(&c->d_total, sizeof(uint64_t)));
+  if (const int rc = c->d_total.alloc(1)) return rc;
   if (const char *e = getenv("OMVG_MATCH_K12_MB")) c->k12_budget_bytes = size_t(atol(e)) << 20;
-  *out = c; return OMVG_OK;
+  *out = c.release(); return OMVG_OK;
 }
 
 int omvg_match_destroy(omvg_match_ctx *c) {
   if (!c) return OMVG_OK;
-  cudaSetDevice(c->device); cudaStreamSynchronize(c->stream);
+  cudaSetDevice(c->device);
+  if (c->stream) cudaStreamSynchronize(c->stream);
   drain_timers(c); for (auto e : c->ev_pool) cudaEventDestroy(e);
-  free_images(c);
-  cudaFree(c->d_k12); cudaFree(c->d_units); cudaFree(c->d_pairs); cudaFree(c->d_counts); cudaFree(c->d_offsets);
-  cudaFree(c->d_total); cudaFree(c->d_out); cudaFree(c->d_models);
-  if (c->h_offsets) cudaFreeHost(c->h_offsets); if (c->h_ij) cudaFreeHost(c->h_ij);
-  cudaStreamDestroy(c->stream);
-  delete c; return OMVG_OK;
+  if (c->stream) cudaStreamDestroy(c->stream);
+  delete c; return OMVG_OK;                               // the buffers release themselves
 }
 
+// On failure the context is left without an image set: every call that needs one returns OMVG_E_STATE.
 int omvg_match_set_images(omvg_match_ctx *c, uint32_t n_images, const uint32_t *counts) {
   if (!c || (!counts && n_images)) return fail(OMVG_E_ARG, "bad arguments");
   OMVG_CUDA(cudaSetDevice(c->device));
   OMVG_CUDA(cudaStreamSynchronize(c->stream));
-  free_images(c);
-  c->n_images = n_images; c->counts.assign(counts, counts + n_images); c->row0.resize(n_images); c->group.resize(n_images);
+  c->img = ImageSet(); c->have_result = false;            // the old set is released before the new one is allocated
+  ImageSet s;
+  s.n_images = n_images; s.counts.assign(counts, counts + n_images); s.row0.resize(n_images); s.group.resize(n_images);
   uint64_t rows = 0; std::vector<uint32_t> row_img;
   for (uint32_t k = 0; k < n_images; ++k) {
-    c->row0[k] = (uint32_t)rows;
+    s.row0[k] = (uint32_t)rows;
     const uint32_t padded = (counts[k] + ROW_PAD - 1) / ROW_PAD * ROW_PAD;
-    c->group[k] = 32 * std::max<uint32_t>(1, (counts[k] + 8191) / 8192);      // rows/group <= 256 groups
-    for (uint32_t s = 0; s < padded / ROW_PAD; ++s) row_img.push_back(k);
+    s.group[k] = 32 * std::max<uint32_t>(1, (counts[k] + 8191) / 8192);      // rows/group <= 256 groups
+    for (uint32_t r = 0; r < padded / ROW_PAD; ++r) row_img.push_back(k);
     rows += padded;
     if (rows + 2 * ROW_PAD > 0xffffffffull) return fail(OMVG_E_ARG, "collection too large (%llu rows)", (unsigned long long)rows);
   }
   rows += ROW_PAD;                                      // tail slot: TMA boxes never leave the arena
   row_img.push_back(n_images ? n_images - 1 : 0);
-  c->total_rows = (uint32_t)rows;
-  OMVG_CUDA(cudaMalloc(&c->d_desc, rows * OMVG_DESC_LEN));
-  OMVG_CUDA(cudaMemsetAsync(c->d_desc, 0, rows * OMVG_DESC_LEN, c->stream));
-  OMVG_CUDA(cudaMalloc(&c->d_norm, rows * 4)); OMVG_CUDA(cudaMalloc(&c->d_ckey, rows * 4));
-  OMVG_CUDA(cudaMalloc(&c->d_dig, rows * DIG_LEN)); OMVG_CUDA(cudaMalloc(&c->d_img_c0, std::max(1u, n_images) * 4)); OMVG_CUDA(cudaMalloc(&c->d_hmm, std::max(1u, n_images) * sizeof(int2)));
-  OMVG_CUDA(cudaMalloc(&c->d_img_row0, std::max(1u, n_images) * 4)); OMVG_CUDA(cudaMalloc(&c->d_img_count, std::max(1u, n_images) * 4));
-  OMVG_CUDA(cudaMalloc(&c->d_img_group, std::max(1u, n_images) * 4)); OMVG_CUDA(cudaMalloc(&c->d_row_img, row_img.size() * 4));
+  s.total_rows = (uint32_t)rows;
+  const size_t ni = std::max(1u, n_images);
+  int rc;
+  if ((rc = s.d_desc.alloc(rows * OMVG_DESC_LEN)) || (rc = s.d_norm.alloc(rows)) || (rc = s.d_ckey.alloc(rows)) ||
+      (rc = s.d_dig.alloc(rows * DIG_LEN / sizeof(uint4))) || (rc = s.d_img_c0.alloc(ni)) || (rc = s.d_hmm.alloc(ni)) ||
+      (rc = s.d_img_row0.alloc(ni)) || (rc = s.d_img_count.alloc(ni)) || (rc = s.d_img_group.alloc(ni)) ||
+      (rc = s.d_row_img.alloc(row_img.size())))
+    return rc;
+  OMVG_CUDA(cudaMemsetAsync(s.d_desc.p, 0, rows * OMVG_DESC_LEN, c->stream));
   if (n_images) {
-    OMVG_CUDA(cudaMemcpyAsync(c->d_img_row0, c->row0.data(), n_images * 4, cudaMemcpyHostToDevice, c->stream));
-    OMVG_CUDA(cudaMemcpyAsync(c->d_img_count, c->counts.data(), n_images * 4, cudaMemcpyHostToDevice, c->stream));
-    OMVG_CUDA(cudaMemcpyAsync(c->d_img_group, c->group.data(), n_images * 4, cudaMemcpyHostToDevice, c->stream));
+    OMVG_CUDA(cudaMemcpyAsync(s.d_img_row0.p, s.row0.data(), n_images * 4, cudaMemcpyHostToDevice, c->stream));
+    OMVG_CUDA(cudaMemcpyAsync(s.d_img_count.p, s.counts.data(), n_images * 4, cudaMemcpyHostToDevice, c->stream));
+    OMVG_CUDA(cudaMemcpyAsync(s.d_img_group.p, s.group.data(), n_images * 4, cudaMemcpyHostToDevice, c->stream));
   }
-  OMVG_CUDA(cudaMemcpyAsync(c->d_row_img, row_img.data(), row_img.size() * 4, cudaMemcpyHostToDevice, c->stream));
+  OMVG_CUDA(cudaMemcpyAsync(s.d_row_img.p, row_img.data(), row_img.size() * 4, cudaMemcpyHostToDevice, c->stream));
   OMVG_CUDA(cudaStreamSynchronize(c->stream));
-  c->uploaded = false; c->prepared = false; c->have_result = false;
-  return make_tmap(c);
+  if ((rc = make_tmap(s))) return rc;
+  c->img = std::move(s); return OMVG_OK;
 }
 
 int omvg_match_upload_host(omvg_match_ctx *c, uint32_t image, const uint8_t *desc) {
-  if (!c || image >= c->n_images || (!desc && c->counts[image])) return fail(OMVG_E_ARG, "bad image %u", image);
-  OMVG_CUDA(cudaSetDevice(c->device));
-  if (c->counts[image])
-    OMVG_CUDA(cudaMemcpyAsync(c->d_desc + (size_t)c->row0[image] * OMVG_DESC_LEN, desc, (size_t)c->counts[image] * OMVG_DESC_LEN,
-                              cudaMemcpyHostToDevice, c->stream));
-  c->uploaded = true; c->prepared = false; c->cascade_ready = false; return OMVG_OK;
+  return upload_desc(c, image, desc, cudaMemcpyHostToDevice);
 }
 
 int omvg_match_upload_device(omvg_match_ctx *c, uint32_t image, const void *desc_dev) {
-  if (!c || image >= c->n_images || (!desc_dev && c->counts[image])) return fail(OMVG_E_ARG, "bad image %u", image);
-  OMVG_CUDA(cudaSetDevice(c->device));
-  if (c->counts[image])
-    OMVG_CUDA(cudaMemcpyAsync(c->d_desc + (size_t)c->row0[image] * OMVG_DESC_LEN, desc_dev, (size_t)c->counts[image] * OMVG_DESC_LEN,
-                              cudaMemcpyDeviceToDevice, c->stream));
-  c->uploaded = true; c->prepared = false; c->cascade_ready = false; return OMVG_OK;
+  return upload_desc(c, image, desc_dev, cudaMemcpyDeviceToDevice);
 }
 
 int omvg_match_upload_device_packed(omvg_match_ctx *c, const void *desc_dev) {
   if (!c || !desc_dev) return fail(OMVG_E_ARG, "bad arguments");
+  if (!c->img.loaded()) return fail(OMVG_E_STATE, "set_images first");
   size_t off = 0;
-  for (uint32_t k = 0; k < c->n_images; ++k) {
+  for (uint32_t k = 0; k < c->img.n_images; ++k) {
     const int rc = omvg_match_upload_device(c, k, static_cast<const uint8_t *>(desc_dev) + off);
     if (rc) return rc;
-    off += (size_t)c->counts[k] * OMVG_DESC_LEN;
+    off += (size_t)c->img.counts[k] * OMVG_DESC_LEN;
   }
-  c->uploaded = true; return OMVG_OK;
+  return OMVG_OK;
 }
 
 int omvg_match_prepare(omvg_match_ctx *c) {
-  if (!c || !c->d_desc) return fail(OMVG_E_STATE, "set_images first");
+  if (!c || !c->img.loaded()) return fail(OMVG_E_STATE, "set_images first");
+  ImageSet &im = c->img;
   OMVG_CUDA(cudaSetDevice(c->device));
   const uint32_t threads = 256, rows_per_block = threads / 8;
-  prep_rows_kernel<<<(c->total_rows + rows_per_block - 1) / rows_per_block, threads, 0, c->stream>>>(
-      c->d_desc, c->d_img_row0, c->d_img_count, c->d_img_group, c->d_row_img, c->d_norm, c->d_ckey, c->total_rows);
-  OMVG_CUDA(cudaGetLastError());
-  c->launches++;
+  int rc;
+  if ((rc = launch(c, prep_rows_kernel, (im.total_rows + rows_per_block - 1) / rows_per_block, threads, 0,
+                   im.d_desc.p, im.d_img_row0.p, im.d_img_count.p, im.d_img_group.p, im.d_row_img.p, im.d_norm.p, im.d_ckey.p, im.total_rows)))
+    return rc;
   // fifth-slice kernel: per-image range of h = ceil(|b|^2 / 2) -> offset c0 and eligibility (one small read-back)
-  c->c0.assign(c->n_images, 0); c->use_dig = false;
+  im.c0.assign(im.n_images, 0); im.use_dig = false;
   const bool force_tc4 = getenv("OMVG_MATCH_TC4") != nullptr;         // A/B: the key-arithmetic variant
-  if (c->n_images && !force_tc4) {
-    prep_minmax_kernel<<<c->n_images, 256, 0, c->stream>>>(c->d_norm, c->d_img_row0, c->d_img_count, c->d_hmm); OMVG_CUDA(cudaGetLastError());
-    std::vector<int2> hmm(c->n_images);
-    OMVG_CUDA(cudaMemcpyAsync(hmm.data(), c->d_hmm, c->n_images * sizeof(int2), cudaMemcpyDeviceToHost, c->stream));
+  if (im.n_images && !force_tc4) {
+    if ((rc = launch(c, prep_minmax_kernel, im.n_images, 256, 0, im.d_norm.p, im.d_img_row0.p, im.d_img_count.p, im.d_hmm.p))) return rc;
+    std::vector<int2> hmm(im.n_images);
+    OMVG_CUDA(cudaMemcpyAsync(hmm.data(), im.d_hmm.p, im.n_images * sizeof(int2), cudaMemcpyDeviceToHost, c->stream));
     OMVG_CUDA(cudaStreamSynchronize(c->stream));
     bool ok = true;
-    for (uint32_t k = 0; k < c->n_images; ++k) {
-      if (!c->counts[k]) continue;
-      if ((long long)hmm[k].y - hmm[k].x > DIG_SPREAD_MAX || c->group[k] / 32 >= 2048) { ok = false; break; }
-      c->c0[k] = std::max(0, hmm[k].y + DIG_VMIN);                           // v = c0 - h in [DIG_VMIN, DIG_VMAX]
+    for (uint32_t k = 0; k < im.n_images; ++k) {
+      if (!im.counts[k]) continue;
+      if ((long long)hmm[k].y - hmm[k].x > DIG_SPREAD_MAX || im.group[k] / 32 >= 2048) { ok = false; break; }
+      im.c0[k] = std::max(0, hmm[k].y + DIG_VMIN);                           // v = c0 - h in [DIG_VMIN, DIG_VMAX]
     }
     if (ok) {
-      OMVG_CUDA(cudaMemcpyAsync(c->d_img_c0, c->c0.data(), c->n_images * 4, cudaMemcpyHostToDevice, c->stream));
-      prep_digits_kernel<<<(c->total_rows + 255) / 256, 256, 0, c->stream>>>(c->d_norm, c->d_img_row0, c->d_img_count, c->d_row_img, c->d_img_c0, c->d_dig, c->total_rows);
-      OMVG_CUDA(cudaGetLastError());
-      OMVG_CUDA(cudaStreamSynchronize(c->stream));                            // c->c0 (host vector) is read by the copy above
-      c->launches += 2; c->use_dig = true;
+      OMVG_CUDA(cudaMemcpyAsync(im.d_img_c0.p, im.c0.data(), im.n_images * 4, cudaMemcpyHostToDevice, c->stream));
+      if ((rc = launch(c, prep_digits_kernel, (im.total_rows + 255) / 256, 256, 0, im.d_norm.p, im.d_img_row0.p, im.d_img_count.p,
+                       im.d_row_img.p, im.d_img_c0.p, im.d_dig.p, im.total_rows)))
+        return rc;
+      OMVG_CUDA(cudaStreamSynchronize(c->stream));                            // im.c0 (host vector) is read by the copy above
+      im.use_dig = true;
     }
   }
-  c->prepared = true; c->cascade_ready = false; return OMVG_OK;
+  im.prepared = true; im.cascade_ready = false; return OMVG_OK;
 }
 
 int omvg_match_run(omvg_match_ctx *c, const uint32_t *pair_i, const uint32_t *pair_j, uint64_t n_pairs, float dist_ratio) {
   if (!c || ((!pair_i || !pair_j) && n_pairs)) return fail(OMVG_E_ARG, "bad arguments");
-  if (!c->prepared) return fail(OMVG_E_STATE, "omvg_match_prepare must follow the uploads");
+  if (!c->img.prepared) return fail(OMVG_E_STATE, "omvg_match_prepare must follow the uploads");
   if (!(dist_ratio >= 0.f)) return fail(OMVG_E_ARG, "dist_ratio must be >= 0");
   OMVG_CUDA(cudaSetDevice(c->device));
-  for (uint64_t p = 0; p < n_pairs; ++p)
-    if (pair_i[p] >= c->n_images || pair_j[p] >= c->n_images) return fail(OMVG_E_ARG, "pair %llu out of range", (unsigned long long)p);
+  const ImageSet &im = c->img;
   const float fratio = dist_ratio * dist_ratio;                   // numeric.h:56 Square<float>, regions_matcher.hpp:196
-  if (const int rc = begin_result(c, n_pairs)) return rc;
-  std::vector<Unit> units; std::vector<PairInfo> pinfo;
-  const size_t budget = c->k12_budget_bytes / sizeof(int2);
-  uint64_t p0 = 0;
-  while (p0 < n_pairs) {
-    size_t acc = 0; uint64_t p1 = p0;
-    while (p1 < n_pairs) {
-      const size_t need = size_t((c->counts[pair_j[p1]] + TILE_Q - 1) / TILE_Q) * TILE_Q;
-      if (p1 > p0 && (acc + need > budget || p1 - p0 >= (1u << 20))) break;
-      acc += need; ++p1;
+  // a batch is charged for every pair's padded queries, inactive pairs included
+  auto cost = [&](uint64_t p) { const size_t need = size_t((im.counts[pair_j[p]] + TILE_Q - 1) / TILE_Q) * TILE_Q; return Cost{need, need}; };
+  auto fill = [&](uint64_t p, PairInfo &P) -> size_t {
+    const uint32_t I = pair_i[p], J = pair_j[p];
+    P.db_row0 = im.row0[I]; P.db_count = im.counts[I]; P.db_group = im.group[I]; P.db_c0 = im.c0[I];
+    P.q_row0 = im.row0[J]; P.q_count = im.counts[J];
+    // Matcher_Regions.cpp:65-69,85-90 (empty regions) and matcher_brute_force.hpp:108-113 (NN > rows)
+    if (P.db_count < 2) P.q_count = 0;
+    if (!P.q_count) return 0;
+    P.unit0 = (uint32_t)(P.out_off / TILE_Q);                     // one work unit per 128 queries
+    return size_t((P.q_count + TILE_Q - 1) / TILE_Q) * TILE_Q;
+  };
+  auto launches = [&](uint64_t, uint32_t nb, size_t rows, uint32_t) {
+    const size_t n_units = rows / TILE_Q;
+    int rc;
+    if (n_units) {
+      if ((rc = c->d_units.reserve(n_units)) || (rc = launch(c, expand_units_kernel, nb, 64, 0, c->d_pairs.p, c->d_units.p))) return rc;
+      const uint32_t grid = (uint32_t)std::min<size_t>(n_units, (size_t)c->n_sms);
+      if ((rc = im.use_dig ? timed_launch(c, match_wgmma_kernel<true>, grid, MATCH_THREADS, match_smem_bytes<true>(), im.tmap, im.tmap_dig, im.d_ckey.p, c->d_units.p, (uint32_t)n_units, c->d_k12.p)
+                           : timed_launch(c, match_wgmma_kernel<false>, grid, MATCH_THREADS, match_smem_bytes<false>(), im.tmap, im.tmap_dig, im.d_ckey.p, c->d_units.p, (uint32_t)n_units, c->d_k12.p)))
+        return rc;
     }
-    const int rc = run_batch(c, pair_i, pair_j, p0, p1, fratio, units, pinfo);
-    if (rc) return rc;
-    p0 = p1;
-  }
-  c->have_result = true; return OMVG_OK;
+    return launch(c, im.use_dig ? match_finalize_kernel<true> : match_finalize_kernel<false>, nb, FIN_THREADS, 0,
+                  im.d_desc.p, im.d_norm.p, c->d_pairs.p, c->d_k12.p, c->d_counts.p, fratio);
+  };
+  return run_pairs(c, pair_i, pair_j, n_pairs, 1u << 20, cost, fill, launches);
 }
 
 int omvg_match_sync(omvg_match_ctx *c) {
@@ -1194,23 +1184,20 @@ int omvg_match_fetch(omvg_match_ctx *c, const uint64_t **offsets, const uint32_t
   if (!c || !offsets || !ij || !n_matches) return fail(OMVG_E_ARG, "bad arguments");
   if (!c->have_result) return fail(OMVG_E_STATE, "no result: call omvg_match_run");
   OMVG_CUDA(cudaSetDevice(c->device));
-  const size_t no = c->n_pairs_last + 1;
-  if (no > c->h_offsets_cap) { if (c->h_offsets) cudaFreeHost(c->h_offsets); c->h_offsets = nullptr; c->h_offsets_cap = 0;
-    OMVG_CUDA(cudaMallocHost(&c->h_offsets, no * sizeof(uint64_t))); c->h_offsets_cap = no; }
-  OMVG_CUDA(cudaMemcpyAsync(c->h_offsets, c->d_offsets, no * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
-  if (c->n_pairs_last == 0) { OMVG_CUDA(cudaStreamSynchronize(c->stream)); c->h_offsets[0] = 0; }
-  const size_t nm = c->total_last;
-  if (nm > c->h_ij_cap || !c->h_ij) { if (c->h_ij) cudaFreeHost(c->h_ij); c->h_ij = nullptr; c->h_ij_cap = 0;
-    OMVG_CUDA(cudaMallocHost(&c->h_ij, std::max<size_t>(nm, 1) * 2 * sizeof(uint32_t))); c->h_ij_cap = std::max<size_t>(nm, 1); }
-  if (nm) OMVG_CUDA(cudaMemcpyAsync(c->h_ij, c->d_out, nm * sizeof(uint2), cudaMemcpyDeviceToHost, c->stream));
+  const size_t no = c->n_pairs_last + 1, nm = c->total_last;
+  int rc;
+  if ((rc = c->h_offsets.reserve(no)) || (rc = c->h_ij.reserve(std::max<size_t>(nm, 1)))) return rc;
+  OMVG_CUDA(cudaMemcpyAsync(c->h_offsets.p, c->d_offsets.p, no * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
+  if (c->n_pairs_last == 0) { OMVG_CUDA(cudaStreamSynchronize(c->stream)); c->h_offsets.p[0] = 0; }
+  if (nm) OMVG_CUDA(cudaMemcpyAsync(c->h_ij.p, c->d_out.p, nm * sizeof(uint2), cudaMemcpyDeviceToHost, c->stream));
   OMVG_CUDA(cudaStreamSynchronize(c->stream));
   drain_timers(c);
-  *offsets = c->h_offsets; *ij = c->h_ij; *n_matches = nm;
+  *offsets = c->h_offsets.p; *ij = reinterpret_cast<const uint32_t *>(c->h_ij.p); *n_matches = nm;
   return OMVG_OK;
 }
 
 uint64_t omvg_match_launch_count(const omvg_match_ctx *c) { return c ? c->launches : 0; }
-int omvg_match_kernel_variant(const omvg_match_ctx *c) { return (!c || !c->prepared) ? 0 : (c->use_dig ? 5 : 4); }
+int omvg_match_kernel_variant(const omvg_match_ctx *c) { return (!c || !c->img.prepared) ? 0 : (c->img.use_dig ? 5 : 4); }
 
 int omvg_match_kernel_time(omvg_match_ctx *c, double *ms, uint64_t *launches, int reset) {
   if (!c) return fail(OMVG_E_ARG, "null ctx");
@@ -1226,116 +1213,105 @@ int omvg_match_kernel_time(omvg_match_ctx *c, double *ms, uint64_t *launches, in
 // 6 x 1024 bucket tables of every image with one radix sort.  Needs omvg_match_prepare (row norms).
 int omvg_match_cascade_prepare(omvg_match_ctx *c, const float *primary, const float *secondary, const uint8_t *used) {
   if (!c || !primary || !secondary) return fail(OMVG_E_ARG, "bad arguments");
-  if (!c->prepared) return fail(OMVG_E_STATE, "omvg_match_prepare must come first");
+  if (!c->img.prepared) return fail(OMVG_E_STATE, "omvg_match_prepare must come first");
+  ImageSet &im = c->img;
   OMVG_CUDA(cudaSetDevice(c->device));
   cudaStream_t st = c->stream;
-  const uint32_t ni = c->n_images;
-  for (uint32_t k = 0; k < ni; ++k) if (c->counts[k] >= (1u << 24)) return fail(OMVG_E_UNSUPPORTED, "image %u has more than 2^24 descriptors", k);
+  const uint32_t ni = im.n_images;
+  for (uint32_t k = 0; k < ni; ++k) if (im.counts[k] >= (1u << 24)) return fail(OMVG_E_UNSUPPORTED, "image %u has more than 2^24 descriptors", k);
+  im.cascade_ready = false;
+  int rc;
   // zero-mean descriptor: exact integer column sums on the device, the two float reductions on the host
   // (float(sum)/float(n) per image; sequential float sum over the used images, / n_used: cascade_hasher.hpp:166-176)
-  unsigned long long *d_sums = nullptr; OMVG_CUDA(cudaMalloc(&d_sums, std::max<size_t>(1, ni) * OMVG_DESC_LEN * sizeof(unsigned long long)));
-  if (ni) { cascade_colsum_kernel<<<ni, OMVG_DESC_LEN, 0, st>>>(c->d_desc, c->d_img_row0, c->d_img_count, d_sums); OMVG_CUDA(cudaGetLastError()); c->launches++; }
   std::vector<unsigned long long> sums((size_t)ni * OMVG_DESC_LEN);
-  if (ni) OMVG_CUDA(cudaMemcpyAsync(sums.data(), d_sums, sums.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  OMVG_CUDA(cudaStreamSynchronize(st)); cudaFree(d_sums);
-  c->h_zm.assign(OMVG_DESC_LEN, 0.0f);
+  {
+    Buf<unsigned long long> d_sums;
+    if ((rc = d_sums.alloc(std::max<size_t>(1, ni) * OMVG_DESC_LEN))) return rc;
+    if (ni) {
+      if ((rc = launch(c, cascade_colsum_kernel, ni, OMVG_DESC_LEN, 0, im.d_desc.p, im.d_img_row0.p, im.d_img_count.p, d_sums.p))) return rc;
+      OMVG_CUDA(cudaMemcpyAsync(sums.data(), d_sums.p, sums.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    }
+    OMVG_CUDA(cudaStreamSynchronize(st));
+  }
+  im.h_zm.assign(OMVG_DESC_LEN, 0.0f);
   uint32_t n_used = 0; for (uint32_t k = 0; k < ni; ++k) if (!used || used[k]) ++n_used;
   for (int col = 0; col < OMVG_DESC_LEN; ++col) {
     float acc = 0.0f;
     for (uint32_t k = 0; k < ni; ++k) { if (used && !used[k]) continue;
-      const float m = c->counts[k] ? (float)sums[(size_t)k * OMVG_DESC_LEN + col] / (float)c->counts[k] : 0.0f; acc = acc + m; }
-    c->h_zm[col] = n_used ? acc / (float)n_used : 0.0f;
+      const float m = im.counts[k] ? (float)sums[(size_t)k * OMVG_DESC_LEN + col] / (float)im.counts[k] : 0.0f; acc = acc + m; }
+    im.h_zm[col] = n_used ? acc / (float)n_used : 0.0f;
   }
-  if (!c->d_proj) OMVG_CUDA(cudaMalloc(&c->d_proj, (size_t)CH_OUT * OMVG_DESC_LEN * sizeof(float)));
-  if (!c->d_zm) OMVG_CUDA(cudaMalloc(&c->d_zm, OMVG_DESC_LEN * sizeof(float)));
-  OMVG_CUDA(cudaMemcpyAsync(c->d_proj, primary, (size_t)OMVG_DESC_LEN * OMVG_DESC_LEN * sizeof(float), cudaMemcpyHostToDevice, st));
-  OMVG_CUDA(cudaMemcpyAsync(c->d_proj + (size_t)OMVG_DESC_LEN * OMVG_DESC_LEN, secondary, (size_t)CH_GROUPS * CH_BITS * OMVG_DESC_LEN * sizeof(float), cudaMemcpyHostToDevice, st));
-  OMVG_CUDA(cudaMemcpyAsync(c->d_zm, c->h_zm.data(), OMVG_DESC_LEN * sizeof(float), cudaMemcpyHostToDevice, st));
-  if (!c->d_code) { OMVG_CUDA(cudaMalloc(&c->d_code, (size_t)c->total_rows * sizeof(uint4))); OMVG_CUDA(cudaMalloc(&c->d_bid, (size_t)c->total_rows * sizeof(uint4))); }
-  cascade_hash_kernel<<<(c->total_rows + CH_HASH_ROWS - 1) / CH_HASH_ROWS, CH_HASH_THREADS, 0, st>>>(c->d_desc, c->total_rows, c->d_zm, c->d_proj, c->d_code, c->d_bid);
-  OMVG_CUDA(cudaGetLastError()); c->launches++;
+  if ((rc = im.d_proj.reserve((size_t)CH_OUT * OMVG_DESC_LEN)) || (rc = im.d_zm.reserve(OMVG_DESC_LEN))) return rc;
+  OMVG_CUDA(cudaMemcpyAsync(im.d_proj.p, primary, (size_t)OMVG_DESC_LEN * OMVG_DESC_LEN * sizeof(float), cudaMemcpyHostToDevice, st));
+  OMVG_CUDA(cudaMemcpyAsync(im.d_proj.p + (size_t)OMVG_DESC_LEN * OMVG_DESC_LEN, secondary, (size_t)CH_GROUPS * CH_BITS * OMVG_DESC_LEN * sizeof(float), cudaMemcpyHostToDevice, st));
+  OMVG_CUDA(cudaMemcpyAsync(im.d_zm.p, im.h_zm.data(), OMVG_DESC_LEN * sizeof(float), cudaMemcpyHostToDevice, st));
+  if ((rc = im.d_code.reserve(im.total_rows)) || (rc = im.d_bid.reserve(im.total_rows))) return rc;
+  if ((rc = launch(c, cascade_hash_kernel, (im.total_rows + CH_HASH_ROWS - 1) / CH_HASH_ROWS, CH_HASH_THREADS, 0,
+                   im.d_desc.p, im.total_rows, im.d_zm.p, im.d_proj.p, im.d_code.p, im.d_bid.p)))
+    return rc;
   // bucket tables
-  std::vector<uint32_t> real0(ni + 1, 0); for (uint32_t k = 0; k < ni; ++k) real0[k + 1] = real0[k] + c->counts[k];
+  std::vector<uint32_t> real0(ni + 1, 0); for (uint32_t k = 0; k < ni; ++k) real0[k + 1] = real0[k] + im.counts[k];
   const uint64_t n_real = real0[ni], n_keys = n_real * CH_GROUPS; const uint32_t n_buckets = ni * CH_GROUPS * CH_NB;
   if (n_keys >= (1ull << 31)) return fail(OMVG_E_UNSUPPORTED, "collection too large for the bucket tables (%llu keys; CUB radix sort takes int counts)", (unsigned long long)n_keys);
-  cudaFree(c->d_bstart); cudaFree(c->d_bitems); c->d_bstart = c->d_bitems = nullptr;
-  OMVG_CUDA(cudaMalloc(&c->d_bstart, ((size_t)n_buckets + 1) * sizeof(uint32_t))); OMVG_CUDA(cudaMalloc(&c->d_bitems, std::max<uint64_t>(1, n_keys) * sizeof(uint32_t)));
-  uint32_t *d_real0 = nullptr; unsigned long long *d_keys = nullptr, *d_keys2 = nullptr; void *d_tmp = nullptr;
-  struct Scratch { uint32_t *&a; unsigned long long *&b, *&c; void *&d; ~Scratch() { cudaFree(a); cudaFree(b); cudaFree(c); cudaFree(d); } } scratch{d_real0, d_keys, d_keys2, d_tmp};   // freed on every exit
-  OMVG_CUDA(cudaMalloc(&d_real0, (ni + 1) * sizeof(uint32_t)));
-  OMVG_CUDA(cudaMemcpyAsync(d_real0, real0.data(), (ni + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-  OMVG_CUDA(cudaMalloc(&d_keys, std::max<uint64_t>(1, n_keys) * 8)); OMVG_CUDA(cudaMalloc(&d_keys2, std::max<uint64_t>(1, n_keys) * 8));
+  Buf<uint32_t> d_real0; Buf<unsigned long long> d_keys, d_keys2; Buf<uint8_t> d_tmp;
+  if ((rc = im.d_bstart.alloc((size_t)n_buckets + 1)) || (rc = im.d_bitems.alloc(std::max<uint64_t>(1, n_keys))) ||
+      (rc = d_real0.alloc(ni + 1)) || (rc = d_keys.alloc(std::max<uint64_t>(1, n_keys))) || (rc = d_keys2.alloc(std::max<uint64_t>(1, n_keys))))
+    return rc;
+  OMVG_CUDA(cudaMemcpyAsync(d_real0.p, real0.data(), (ni + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
   if (n_keys) {
-    cascade_keys_kernel<<<dim3(32, ni), 256, 0, st>>>(c->d_bid, c->d_img_row0, c->d_img_count, d_real0, ni, d_keys); OMVG_CUDA(cudaGetLastError());
+    if ((rc = launch(c, cascade_keys_kernel, dim3(32, ni), 256, 0, im.d_bid.p, im.d_img_row0.p, im.d_img_count.p, d_real0.p, ni, d_keys.p))) return rc;
     int seg_bits = 1; while ((1ull << seg_bits) < (unsigned long long)ni * CH_GROUPS) ++seg_bits;
-    size_t tb = 0; OMVG_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb, d_keys, d_keys2, (int)n_keys, 0, 34 + seg_bits, st));
-    OMVG_CUDA(cudaMalloc(&d_tmp, tb));
-    OMVG_CUDA(cub::DeviceRadixSort::SortKeys(d_tmp, tb, d_keys, d_keys2, (int)n_keys, 0, 34 + seg_bits, st));
-    c->launches += 2;
+    size_t tb = 0; OMVG_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb, d_keys.p, d_keys2.p, (int)n_keys, 0, 34 + seg_bits, st));
+    if ((rc = d_tmp.alloc(tb))) return rc;
+    OMVG_CUDA(cub::DeviceRadixSort::SortKeys(d_tmp.p, tb, d_keys.p, d_keys2.p, (int)n_keys, 0, 34 + seg_bits, st));
+    c->launches++;                                                            // the sort counts as one launch
   }
-  cascade_starts_kernel<<<(unsigned)((n_keys + 256) / 256), 256, 0, st>>>(d_keys2, n_keys, n_buckets, c->d_bstart, c->d_bitems); OMVG_CUDA(cudaGetLastError());
-  c->launches++;
+  if ((rc = launch(c, cascade_starts_kernel, (unsigned)((n_keys + 256) / 256), 256, 0, d_keys2.p, n_keys, n_buckets, im.d_bstart.p, im.d_bitems.p))) return rc;
   OMVG_CUDA(cudaStreamSynchronize(st));
-  c->cascade_ready = true; return OMVG_OK;
+  im.cascade_ready = true; return OMVG_OK;
 }
 
 // Cascade_Hashing_Matcher_Regions.cpp:110-189 for a list of pairs (I = database, J = queries).  The result is read
 // with omvg_match_fetch: CSR rows of (i, j) in ascending j (the caller sorts by (i, j) as IndMatch::getDeduplicated does).
 int omvg_match_cascade_run(omvg_match_ctx *c, const uint32_t *pair_i, const uint32_t *pair_j, uint64_t n_pairs, float dist_ratio) {
   if (!c || ((!pair_i || !pair_j) && n_pairs)) return fail(OMVG_E_ARG, "bad arguments");
-  if (!c->cascade_ready) return fail(OMVG_E_STATE, "omvg_match_cascade_prepare first");
+  if (!c->img.cascade_ready) return fail(OMVG_E_STATE, "omvg_match_cascade_prepare first");
   if (!(dist_ratio >= 0.f)) return fail(OMVG_E_ARG, "dist_ratio must be >= 0");
   OMVG_CUDA(cudaSetDevice(c->device));
-  for (uint64_t p = 0; p < n_pairs; ++p)
-    if (pair_i[p] >= c->n_images || pair_j[p] >= c->n_images) return fail(OMVG_E_ARG, "pair %llu out of range", (unsigned long long)p);
+  const ImageSet &im = c->img;
   const float fratio = dist_ratio * dist_ratio;
-  if (const int rc = begin_result(c, n_pairs)) return rc;
-  std::vector<PairInfo> pinfo;
-  const size_t budget = c->k12_budget_bytes / sizeof(int2);
-  uint64_t p0 = 0;
-  while (p0 < n_pairs) {
-    pinfo.clear(); size_t out = 0; uint64_t p1 = p0; uint32_t maxq = 0;
-    while (p1 < n_pairs && p1 - p0 < 65535) {
-      const uint32_t I = pair_i[p1], J = pair_j[p1];
-      if (p1 > p0 && out + c->counts[J] > budget) break;
-      PairInfo P{}; P.db_row0 = c->row0[I]; P.db_count = c->counts[I]; P.db_group = I; P.q_row0 = c->row0[J]; P.q_count = c->counts[J]; P.out_off = out;
-      if (P.db_count == 0) P.q_count = 0;                      // empty database image: nothing (:120-124)
-      out += P.q_count; maxq = std::max(maxq, P.q_count); pinfo.push_back(P); ++p1;
-    }
-    const uint32_t nb = (uint32_t)(p1 - p0);
+  // a pair needs room for all of J's queries but takes none for an empty database image (:120-124)
+  auto cost = [&](uint64_t p) { const uint32_t nq = im.counts[pair_j[p]]; return Cost{nq, im.counts[pair_i[p]] ? nq : 0}; };
+  auto fill = [&](uint64_t p, PairInfo &P) -> size_t {
+    const uint32_t I = pair_i[p], J = pair_j[p];
+    P.db_row0 = im.row0[I]; P.db_count = im.counts[I]; P.db_group = I; P.q_row0 = im.row0[J];
+    P.q_count = P.db_count ? im.counts[J] : 0;
+    return P.q_count;
+  };
+  auto launches = [&](uint64_t, uint32_t nb, size_t, uint32_t maxq) {
     int rc;
-    if ((rc = ensure(c->d_k12, c->k12_cap, std::max<size_t>(out, 1)))) return rc;
-    if ((rc = ensure_pairs(c, nb))) return rc;
-    OMVG_CUDA(cudaMemcpyAsync(c->d_pairs, pinfo.data(), nb * sizeof(PairInfo), cudaMemcpyHostToDevice, c->stream));
-    if (maxq) {
-      cudaEvent_t e0 = get_event(c), e1 = get_event(c);
-      OMVG_CUDA(cudaEventRecord(e0, c->stream));
-      cascade_query_kernel<<<dim3((maxq + 31) / 32, nb), 256, 0, c->stream>>>(c->d_desc, c->d_norm, c->d_code, c->d_bid, c->d_bstart, c->d_bitems, c->d_pairs, c->d_k12, fratio);
-      OMVG_CUDA(cudaGetLastError());
-      OMVG_CUDA(cudaEventRecord(e1, c->stream));
-      c->pending.emplace_back(e0, e1); c->tc_launches++; c->launches++;
-    }
-    cascade_compact_kernel<<<nb, FIN_THREADS, 0, c->stream>>>(c->d_pairs, c->d_k12, c->d_counts); OMVG_CUDA(cudaGetLastError());
-    c->launches++;
-    if ((rc = gather_batch(c, nb, p0))) return rc;
-    p0 = p1;
-  }
-  c->have_result = true; return OMVG_OK;
+    if (maxq && (rc = timed_launch(c, cascade_query_kernel, dim3((maxq + 31) / 32, nb), 256, 0, im.d_desc.p, im.d_norm.p, im.d_code.p, im.d_bid.p,
+                                   im.d_bstart.p, im.d_bitems.p, c->d_pairs.p, c->d_k12.p, fratio)))
+      return rc;
+    return launch(c, cascade_compact_kernel, nb, FIN_THREADS, 0, c->d_pairs.p, c->d_k12.p, c->d_counts.p);
+  };
+  return run_pairs(c, pair_i, pair_j, n_pairs, 65535, cost, fill, launches);
 }
 
 // ---- guided matching ---------------------------------------------------------------------------------------
 int omvg_match_upload_positions(omvg_match_ctx *c, uint32_t image, const double *xy) {
   if (!c) return fail(OMVG_E_ARG, "null ctx");
-  if (!c->d_desc) return fail(OMVG_E_STATE, "set_images first");
-  if (image >= c->n_images || (!xy && c->counts[image])) return fail(OMVG_E_ARG, "bad image %u", image);
+  ImageSet &im = c->img;
+  if (!im.loaded()) return fail(OMVG_E_STATE, "set_images first");
+  if (image >= im.n_images || (!xy && im.counts[image])) return fail(OMVG_E_ARG, "bad image %u", image);
   OMVG_CUDA(cudaSetDevice(c->device));
-  if (!c->d_pos) {
-    OMVG_CUDA(cudaMalloc(&c->d_pos, (size_t)c->total_rows * sizeof(double2)));
-    c->has_pos.assign(c->n_images, 0);
+  if (!im.d_pos.p) {
+    if (const int rc = im.d_pos.alloc(im.total_rows)) return rc;
+    im.has_pos.assign(im.n_images, 0);
   }
-  if (c->counts[image])
-    OMVG_CUDA(cudaMemcpyAsync(c->d_pos + c->row0[image], xy, (size_t)c->counts[image] * sizeof(double2), cudaMemcpyHostToDevice, c->stream));
-  c->has_pos[image] = 1;
+  if (im.counts[image])
+    OMVG_CUDA(cudaMemcpyAsync(im.d_pos.p + im.row0[image], xy, (size_t)im.counts[image] * sizeof(double2), cudaMemcpyHostToDevice, c->stream));
+  im.has_pos[image] = 1;
   return OMVG_OK;
 }
 
@@ -1345,115 +1321,105 @@ int omvg_match_guided_run(omvg_match_ctx *c, int32_t error_model, const uint32_t
   if (!c || ((!pair_i || !pair_j || !models || !thresholds) && n_pairs)) return fail(OMVG_E_ARG, "bad arguments");
   if (error_model != OMVG_GUIDED_EPIPOLAR && error_model != OMVG_GUIDED_TRANSFER) return fail(OMVG_E_ARG, "unknown error model %d", error_model);
   if (std::isnan(dist_ratio)) return fail(OMVG_E_ARG, "dist_ratio is NaN");
-  if (!c->prepared) return fail(OMVG_E_STATE, "omvg_match_prepare must follow the uploads");
+  if (!c->img.prepared) return fail(OMVG_E_STATE, "omvg_match_prepare must follow the uploads");
+  const ImageSet &im = c->img;
   for (uint64_t p = 0; p < n_pairs; ++p) {
-    if (pair_i[p] >= c->n_images || pair_j[p] >= c->n_images) return fail(OMVG_E_ARG, "pair %llu out of range", (unsigned long long)p);
-    if (c->has_pos.empty() || !c->has_pos[pair_i[p]] || !c->has_pos[pair_j[p]]) return fail(OMVG_E_STATE, "pair %llu: an image has no positions", (unsigned long long)p);
+    if (pair_i[p] >= im.n_images || pair_j[p] >= im.n_images) return fail(OMVG_E_ARG, "pair %llu out of range", (unsigned long long)p);
+    if (im.has_pos.empty() || !im.has_pos[pair_i[p]] || !im.has_pos[pair_j[p]]) return fail(OMVG_E_STATE, "pair %llu: an image has no positions", (unsigned long long)p);
     bool finite = std::isfinite(thresholds[p]);
     for (int k = 0; k < 9; ++k) finite = finite && std::isfinite(models[9 * p + k]);
     if (!finite) return fail(OMVG_E_ARG, "pair %llu: non-finite model or threshold", (unsigned long long)p);
   }
   OMVG_CUDA(cudaSetDevice(c->device));
-  if (const int rc = begin_result(c, n_pairs)) return rc;
   const bool desc = dist_ratio >= 0.0;
-  std::vector<PairInfo> pinfo; std::vector<GuidedModel> gm;
-  const size_t budget = c->k12_budget_bytes / sizeof(int2);
-  uint64_t p0 = 0;
-  while (p0 < n_pairs) {
-    pinfo.clear(); gm.clear(); size_t out = 0; uint64_t p1 = p0; uint32_t maxq = 0;
-    while (p1 < n_pairs && p1 - p0 < 65535) {
-      const uint32_t I = pair_i[p1], J = pair_j[p1];
-      if (p1 > p0 && out + c->counts[I] > budget) break;
-      PairInfo P{}; P.q_row0 = c->row0[I]; P.q_count = c->counts[I]; P.db_row0 = c->row0[J]; P.db_count = c->counts[J]; P.out_off = out;
-      GuidedModel G; for (int k = 0; k < 9; ++k) G.M[k] = models[9 * p1 + k]; G.thr = thresholds[p1];
-      out += P.q_count; maxq = std::max(maxq, P.q_count); pinfo.push_back(P); gm.push_back(G); ++p1;
-    }
-    const uint32_t nb = (uint32_t)(p1 - p0);
+  auto kernel = error_model == OMVG_GUIDED_EPIPOLAR ? (desc ? guided_match_kernel<OMVG_GUIDED_EPIPOLAR, true> : guided_match_kernel<OMVG_GUIDED_EPIPOLAR, false>)
+                                                    : (desc ? guided_match_kernel<OMVG_GUIDED_TRANSFER, true> : guided_match_kernel<OMVG_GUIDED_TRANSFER, false>);
+  // I's features are the queries
+  auto cost = [&](uint64_t p) { const size_t nq = im.counts[pair_i[p]]; return Cost{nq, nq}; };
+  auto fill = [&](uint64_t p, PairInfo &P) -> size_t {
+    const uint32_t I = pair_i[p], J = pair_j[p];
+    P.q_row0 = im.row0[I]; P.q_count = im.counts[I]; P.db_row0 = im.row0[J]; P.db_count = im.counts[J];
+    return P.q_count;
+  };
+  std::vector<GuidedModel> gm;
+  auto launches = [&](uint64_t p0, uint32_t nb, size_t, uint32_t maxq) {
+    gm.resize(nb);
+    for (uint32_t b = 0; b < nb; ++b) { for (int k = 0; k < 9; ++k) gm[b].M[k] = models[9 * (p0 + b) + k]; gm[b].thr = thresholds[p0 + b]; }
     int rc;
-    if ((rc = ensure(c->d_k12, c->k12_cap, std::max<size_t>(out, 1)))) return rc;
-    if ((rc = ensure_pairs(c, nb))) return rc;
-    if ((rc = ensure(c->d_models, c->models_cap, nb))) return rc;
-    OMVG_CUDA(cudaMemcpyAsync(c->d_pairs, pinfo.data(), nb * sizeof(PairInfo), cudaMemcpyHostToDevice, c->stream));
-    OMVG_CUDA(cudaMemcpyAsync(c->d_models, gm.data(), nb * sizeof(GuidedModel), cudaMemcpyHostToDevice, c->stream));
-    if (maxq) {
-      const dim3 grid((maxq + GM_THREADS - 1) / GM_THREADS, nb);
-      cudaEvent_t e0 = get_event(c), e1 = get_event(c);
-      OMVG_CUDA(cudaEventRecord(e0, c->stream));
-      auto k = error_model == OMVG_GUIDED_EPIPOLAR ? (desc ? guided_match_kernel<OMVG_GUIDED_EPIPOLAR, true> : guided_match_kernel<OMVG_GUIDED_EPIPOLAR, false>)
-                                                   : (desc ? guided_match_kernel<OMVG_GUIDED_TRANSFER, true> : guided_match_kernel<OMVG_GUIDED_TRANSFER, false>);
-      k<<<grid, GM_THREADS, 0, c->stream>>>(c->d_pos, c->d_desc, c->d_norm, c->d_pairs, c->d_models, c->d_k12, dist_ratio);
-      OMVG_CUDA(cudaGetLastError());
-      OMVG_CUDA(cudaEventRecord(e1, c->stream));
-      c->pending.emplace_back(e0, e1); c->tc_launches++; c->launches++;
-    }
-    guided_compact_kernel<<<nb, FIN_THREADS, 0, c->stream>>>(c->d_pairs, c->d_k12, c->d_counts); OMVG_CUDA(cudaGetLastError());
-    c->launches++;
-    if ((rc = gather_batch(c, nb, p0))) return rc;
-    p0 = p1;
-  }
-  c->have_result = true; return OMVG_OK;
+    if ((rc = c->d_models.reserve(nb))) return rc;
+    OMVG_CUDA(cudaMemcpyAsync(c->d_models.p, gm.data(), nb * sizeof(GuidedModel), cudaMemcpyHostToDevice, c->stream));
+    if (maxq && (rc = timed_launch(c, kernel, dim3((maxq + GM_THREADS - 1) / GM_THREADS, nb), GM_THREADS, 0, im.d_pos.p, im.d_desc.p, im.d_norm.p,
+                                   c->d_pairs.p, c->d_models.p, c->d_k12.p, dist_ratio)))
+      return rc;
+    return launch(c, guided_compact_kernel, nb, FIN_THREADS, 0, c->d_pairs.p, c->d_k12.p, c->d_counts.p);
+  };
+  return run_pairs(c, pair_i, pair_j, n_pairs, 65535, cost, fill, launches);
 }
 
 // Validation aid (tests only): hash codes [count][4], bucket ids [count][6] and the zero-mean vector [128].
 int omvg_match_cascade_debug_hash(omvg_match_ctx *c, uint32_t image, uint32_t *codes, uint16_t *bids, float *zero_mean) {
-  if (!c || image >= c->n_images) return fail(OMVG_E_ARG, "bad arguments");
-  if (!c->cascade_ready) return fail(OMVG_E_STATE, "omvg_match_cascade_prepare first");
+  if (!c) return fail(OMVG_E_ARG, "bad arguments");
+  const ImageSet &im = c->img;
+  if (!im.cascade_ready) return fail(OMVG_E_STATE, "omvg_match_cascade_prepare first");
+  if (image >= im.n_images) return fail(OMVG_E_ARG, "bad arguments");
   OMVG_CUDA(cudaSetDevice(c->device));
-  const uint32_t n = c->counts[image];
+  const uint32_t n = im.counts[image];
   std::vector<uint4> hc(n), hb(n);
-  if (n) { OMVG_CUDA(cudaMemcpyAsync(hc.data(), c->d_code + c->row0[image], n * sizeof(uint4), cudaMemcpyDeviceToHost, c->stream));
-           OMVG_CUDA(cudaMemcpyAsync(hb.data(), c->d_bid + c->row0[image], n * sizeof(uint4), cudaMemcpyDeviceToHost, c->stream)); }
+  if (n) { OMVG_CUDA(cudaMemcpyAsync(hc.data(), im.d_code.p + im.row0[image], n * sizeof(uint4), cudaMemcpyDeviceToHost, c->stream));
+           OMVG_CUDA(cudaMemcpyAsync(hb.data(), im.d_bid.p + im.row0[image], n * sizeof(uint4), cudaMemcpyDeviceToHost, c->stream)); }
   OMVG_CUDA(cudaStreamSynchronize(c->stream));
   for (uint32_t r = 0; r < n; ++r) {
     if (codes) { codes[4 * r] = hc[r].x; codes[4 * r + 1] = hc[r].y; codes[4 * r + 2] = hc[r].z; codes[4 * r + 3] = hc[r].w; }
     if (bids) { bids[6 * r] = hb[r].x & 0xffff; bids[6 * r + 1] = hb[r].x >> 16; bids[6 * r + 2] = hb[r].y & 0xffff; bids[6 * r + 3] = hb[r].y >> 16; bids[6 * r + 4] = hb[r].z & 0xffff; bids[6 * r + 5] = hb[r].z >> 16; }
   }
-  if (zero_mean) for (int k = 0; k < OMVG_DESC_LEN; ++k) zero_mean[k] = c->h_zm[k];
+  if (zero_mean) for (int k = 0; k < OMVG_DESC_LEN; ++k) zero_mean[k] = im.h_zm[k];
   return OMVG_OK;
 }
 
 int omvg_match_debug_top2_simt(omvg_match_ctx *c, uint32_t I, uint32_t J, int32_t *d1, uint32_t *i1, int32_t *d2) {
-  if (!c || I >= c->n_images || J >= c->n_images) return fail(OMVG_E_ARG, "bad image");
-  if (!c->prepared) return fail(OMVG_E_STATE, "prepare first");
+  if (!c) return fail(OMVG_E_ARG, "bad image");
+  const ImageSet &im = c->img;
+  if (!im.prepared) return fail(OMVG_E_STATE, "prepare first");
+  if (I >= im.n_images || J >= im.n_images) return fail(OMVG_E_ARG, "bad image");
   OMVG_CUDA(cudaSetDevice(c->device));
-  const uint32_t nq = c->counts[J];
-  if (nq == 0 || c->counts[I] < 2) return fail(OMVG_E_ARG, "need >=2 database rows and >=1 query");
-  int32_t *dd1, *dd2; uint32_t *di1;
-  OMVG_CUDA(cudaMalloc(&dd1, nq * 4)); OMVG_CUDA(cudaMalloc(&dd2, nq * 4)); OMVG_CUDA(cudaMalloc(&di1, nq * 4));
-  top2_simt_kernel<<<nq, 128, 0, c->stream>>>(c->d_desc, c->d_norm, c->row0[I], c->counts[I], c->row0[J], dd1, di1, dd2);
-  OMVG_CUDA(cudaGetLastError()); c->launches++;
-  OMVG_CUDA(cudaMemcpyAsync(d1, dd1, nq * 4, cudaMemcpyDeviceToHost, c->stream));
-  OMVG_CUDA(cudaMemcpyAsync(i1, di1, nq * 4, cudaMemcpyDeviceToHost, c->stream));
-  OMVG_CUDA(cudaMemcpyAsync(d2, dd2, nq * 4, cudaMemcpyDeviceToHost, c->stream));
+  const uint32_t nq = im.counts[J];
+  if (nq == 0 || im.counts[I] < 2) return fail(OMVG_E_ARG, "need >=2 database rows and >=1 query");
+  Buf<int32_t> dd1, dd2; Buf<uint32_t> di1;
+  int rc;
+  if ((rc = dd1.alloc(nq)) || (rc = dd2.alloc(nq)) || (rc = di1.alloc(nq)) ||
+      (rc = launch(c, top2_simt_kernel, nq, 128, 0, im.d_desc.p, im.d_norm.p, im.row0[I], im.counts[I], im.row0[J], dd1.p, di1.p, dd2.p)))
+    return rc;
+  OMVG_CUDA(cudaMemcpyAsync(d1, dd1.p, nq * 4, cudaMemcpyDeviceToHost, c->stream));
+  OMVG_CUDA(cudaMemcpyAsync(i1, di1.p, nq * 4, cudaMemcpyDeviceToHost, c->stream));
+  OMVG_CUDA(cudaMemcpyAsync(d2, dd2.p, nq * 4, cudaMemcpyDeviceToHost, c->stream));
   OMVG_CUDA(cudaStreamSynchronize(c->stream));
-  cudaFree(dd1); cudaFree(dd2); cudaFree(di1);
   return OMVG_OK;
 }
 
 int omvg_match_debug_top2_tc(omvg_match_ctx *c, uint32_t I, uint32_t J, int32_t *d1, uint32_t *g1, int32_t *ub2) {
-  if (!c || I >= c->n_images || J >= c->n_images) return fail(OMVG_E_ARG, "bad image");
-  if (!c->prepared) return fail(OMVG_E_STATE, "prepare first");
+  if (!c) return fail(OMVG_E_ARG, "bad image");
+  const ImageSet &im = c->img;
+  if (!im.prepared) return fail(OMVG_E_STATE, "prepare first");
+  if (I >= im.n_images || J >= im.n_images) return fail(OMVG_E_ARG, "bad image");
   OMVG_CUDA(cudaSetDevice(c->device));
-  const uint32_t nq = c->counts[J], ndb = c->counts[I];
+  const uint32_t nq = im.counts[J], ndb = im.counts[I];
   if (nq == 0 || ndb < 2) return fail(OMVG_E_ARG, "need >=2 database rows and >=1 query");
   const uint32_t qt = (nq + TILE_Q - 1) / TILE_Q, dt = (ndb + TILE_DB - 1) / TILE_DB;
   std::vector<Unit> units;
-  for (uint32_t t = 0; t < qt; ++t) units.push_back(Unit{c->row0[J] + t * TILE_Q, c->row0[I], dt, t * TILE_Q});
+  for (uint32_t t = 0; t < qt; ++t) units.push_back(Unit{im.row0[J] + t * TILE_Q, im.row0[I], dt, t * TILE_Q});
   int rc;
-  if ((rc = ensure(c->d_k12, c->k12_cap, size_t(qt) * TILE_Q))) return rc;
-  if ((rc = ensure(c->d_units, c->units_cap, units.size()))) return rc;
-  OMVG_CUDA(cudaMemcpyAsync(c->d_units, units.data(), units.size() * sizeof(Unit), cudaMemcpyHostToDevice, c->stream));
-  match_wgmma_kernel<false><<<std::min<uint32_t>(qt, c->n_sms), MATCH_THREADS, match_smem_bytes<false>(), c->stream>>>(c->tmap, c->tmap_dig, c->d_ckey, c->d_units, qt, c->d_k12);
-  OMVG_CUDA(cudaGetLastError()); c->launches++;
-  int32_t *dd1, *dd2; uint32_t *dg1;
-  OMVG_CUDA(cudaMalloc(&dd1, nq * 4)); OMVG_CUDA(cudaMalloc(&dd2, nq * 4)); OMVG_CUDA(cudaMalloc(&dg1, nq * 4));
-  decode_k12_kernel<<<(nq + 255) / 256, 256, 0, c->stream>>>(c->d_k12, c->d_norm, c->row0[J], nq, dd1, dg1, dd2);
-  OMVG_CUDA(cudaGetLastError()); c->launches++;
-  OMVG_CUDA(cudaMemcpyAsync(d1, dd1, nq * 4, cudaMemcpyDeviceToHost, c->stream));
-  OMVG_CUDA(cudaMemcpyAsync(g1, dg1, nq * 4, cudaMemcpyDeviceToHost, c->stream));
-  OMVG_CUDA(cudaMemcpyAsync(ub2, dd2, nq * 4, cudaMemcpyDeviceToHost, c->stream));
+  if ((rc = c->d_k12.reserve(size_t(qt) * TILE_Q)) || (rc = c->d_units.reserve(units.size()))) return rc;
+  OMVG_CUDA(cudaMemcpyAsync(c->d_units.p, units.data(), units.size() * sizeof(Unit), cudaMemcpyHostToDevice, c->stream));
+  Buf<int32_t> dd1, dd2; Buf<uint32_t> dg1;
+  if ((rc = launch(c, match_wgmma_kernel<false>, std::min<uint32_t>(qt, c->n_sms), MATCH_THREADS, match_smem_bytes<false>(),
+                   im.tmap, im.tmap_dig, im.d_ckey.p, c->d_units.p, qt, c->d_k12.p)) ||
+      (rc = dd1.alloc(nq)) || (rc = dd2.alloc(nq)) || (rc = dg1.alloc(nq)) ||
+      (rc = launch(c, decode_k12_kernel, (nq + 255) / 256, 256, 0, c->d_k12.p, im.d_norm.p, im.row0[J], nq, dd1.p, dg1.p, dd2.p)))
+    return rc;
+  OMVG_CUDA(cudaMemcpyAsync(d1, dd1.p, nq * 4, cudaMemcpyDeviceToHost, c->stream));
+  OMVG_CUDA(cudaMemcpyAsync(g1, dg1.p, nq * 4, cudaMemcpyDeviceToHost, c->stream));
+  OMVG_CUDA(cudaMemcpyAsync(ub2, dd2.p, nq * 4, cudaMemcpyDeviceToHost, c->stream));
   OMVG_CUDA(cudaStreamSynchronize(c->stream));
-  cudaFree(dd1); cudaFree(dd2); cudaFree(dg1);
   c->have_result = false;
   return OMVG_OK;
 }

@@ -84,17 +84,64 @@ def test_large_database_groups(matching):
     ctx.close()
 
 
-def test_batched_runs_match_single(matching, monkeypatch):
-    """Small k12 budget forces several batches; result must not change."""
-    import os
+def _batched_matches_single(matching, monkeypatch, cascade):
     descs = synth.descriptors(6, [400, 500, 300, 450, 380, 410], seed=4)
     pi, pj = synth.exhaustive_pairs(6)
-    ctx = matching.MatchContext(0)
-    ctx.load(descs); ctx.run(pi, pj, 0.8); off1, ij1 = ctx.fetch(); ctx.close()
+
+    def run():
+        ctx = matching.MatchContext(0)
+        ctx.load(descs)
+        if cascade:
+            ctx.cascade_prepare(*ck.cascade_projections())
+        n0 = ctx.launch_count()
+        (ctx.cascade_run if cascade else ctx.run)(pi, pj, 0.8)
+        n_launches = ctx.launch_count() - n0
+        out = ctx.fetch(); ctx.close()
+        return out, n_launches
+    (off1, ij1), n1 = run()
     monkeypatch.setenv("OMVG_MATCH_K12_MB", "0")        # 0 MB => one pair per batch
-    ctx = matching.MatchContext(0)
-    ctx.load(descs); ctx.run(pi, pj, 0.8); off2, ij2 = ctx.fetch(); ctx.close()
+    (off2, ij2), n2 = run()
+    assert n2 > n1                                      # the second run really was cut into batches
     _csr_equal(off1, ij1, off2, ij2)
+
+
+def test_batched_runs_match_single(matching, monkeypatch):
+    """Small k12 budget forces several batches; result must not change."""
+    _batched_matches_single(matching, monkeypatch, cascade=False)
+
+
+def test_batched_cascade_runs_match_single(matching, monkeypatch):
+    """The same for cascade hashing: one pair per batch gives the CSR of the single-batch run."""
+    _batched_matches_single(matching, monkeypatch, cascade=True)
+
+
+def test_failed_set_images_leaves_no_image_set(matching):
+    """A set_images that fails (here the host-side size check, before any allocation) leaves the context without an
+    image set: every call that needs one reports OMVG_E_STATE, and the next set_images works normally."""
+    import ctypes
+    from openmvg_b200._lib import OmvgError, lib
+    E_ARG, E_STATE = -1, -3
+    ctx = matching.MatchContext(0)
+    with pytest.raises(OmvgError) as e:
+        ctx.set_images([2**31 - 1, 2**31 - 1])
+    assert e.value.code == E_ARG
+    pi, pj = np.array([0], np.uint32), np.array([1], np.uint32)
+    small = np.zeros((4, 128), np.uint8); xy = np.zeros((4, 2))
+    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+    assert lib().omvg_match_upload_host(ctx._h, 0, vp(small)) == E_STATE
+    assert lib().omvg_match_upload_positions(ctx._h, 0, vp(xy)) == E_STATE
+    for call in (ctx.prepare, lambda: ctx.run(pi, pj, 0.8), lambda: ctx.cascade_prepare(*ck.cascade_projections()),
+                 lambda: ctx.guided_run(pi, pj, np.eye(3)[None], [1.0], 0.36)):
+        with pytest.raises(OmvgError) as e:
+            call()
+        assert e.value.code == E_STATE
+    descs = synth.descriptors(3, [300, 450, 200], seed=9)
+    pi, pj = synth.exhaustive_pairs(3)
+    ctx.load(descs); ctx.run(pi, pj, 0.8)
+    off, ij = ctx.fetch()
+    ooff, oij = ck.oracle_match_collection(descs, pi, pj, 0.8)
+    _csr_equal(off, ij, ooff, oij)
+    ctx.close()
 
 
 def test_matcher_interface(matching):
