@@ -342,6 +342,10 @@ int omvg_ba_commit(omvg_ba_ctx *ctx);
  * Huber-corrected, NOT Jacobi-scaled), in the caller's observation order; cost returned. */
 int omvg_ba_debug_eval(omvg_ba_ctx *ctx, const omvg_ba_options *options, double *cost, double *r,
                        double *J_intr, double *J_pose, double *J_point);
+/* Validation aid (tests only): the pose-centre prior rows at the uploaded parameters, as the solve forms them
+ * (Huber-corrected, NOT Jacobi-scaled, masked by options->extrinsics_opt): r[n_priors][3], J[n_priors][3][6] (pose
+ * columns), in the caller's prior order; *cost = 1/2 sum rho of the prior rows alone.  Any pointer may be NULL. */
+int omvg_ba_debug_prior(omvg_ba_ctx *ctx, const omvg_ba_options *options, double *cost, double *r, double *J);
 /* Validation aid (tests only): the first LM step of omvg_ba_run at trust-region radius `radius`, taken apart.  With
  * nd = 6 n_poses + 8 n_intrinsics and nx = 3 n_points + nd (points, then poses, then intrinsic slots):
  *   scale[nx]      Jacobi column scaling of the unscaled J;  lm_diag[nx]  LM diagonal D (D^2 = clamp(diag) / radius)

@@ -194,6 +194,16 @@ class BAContext:
         check(lib().omvg_ba_debug_eval(self._h, ctypes.byref(o), ctypes.byref(cost), d(r), d(Ji), d(Jc), d(Jp)))
         return cost.value, r, Ji, Jc, Jp
 
+    def debug_prior(self, **opts):
+        """The pose-centre prior rows at the uploaded parameters (omvg_ba_debug_prior): (cost, r [n_priors][3],
+        J [n_priors][3][6]), Huber-corrected, unscaled, masked by the extrinsics option."""
+        o = default_options(**opts)
+        pp = self._s.get("prior_pose")
+        n = 0 if pp is None else len(pp)
+        r = np.zeros((n, 3)); J = np.zeros((n, 3, 6)); cost = ctypes.c_double()
+        check(lib().omvg_ba_debug_prior(self._h, ctypes.byref(o), ctypes.byref(cost), r.ctypes.data_as(_dp), J.ctypes.data_as(_dp)))
+        return cost.value, r, J
+
     # solver ids of omvg_ba_debug_step
     SOLVERS = ("dense_ldlt", "dense_inverse", "pcg5", "pcg3", "pcg")
 

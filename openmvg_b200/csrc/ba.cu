@@ -1156,8 +1156,10 @@ int omvg_ba_debug_eval(omvg_ba_ctx *c, const omvg_ba_options *O, double *cost, d
   EvalArgs A; int rc = eval_prep(c, 0, A); if (rc) return rc;
   A.use_loss = O->use_loss; A.huber_a = O->huber_a; A.r = c->r.p; A.Jp = c->Jp.p; A.Jc = c->Jc.p; A.Ji = c->Ji.p;
   A.kiu = c->kiu; A.pose_mask = m.pose_mask; A.intr_mask = c->intr_mask.p; A.pts_free = m.pts_free;
-  A.obs_w = c->obs_w.p; A.obs_flags = c->obs_flags.p; A.pt_fixed = c->pt_fixed.p;      // (prior rows are not part of this dump)
-  if ((rc = launch(c, eval_kernel<true, 4, true>, c->eval_grid, EVAL_THREADS, 0, A)) || (rc = reduce_to(c, c->part.p, c->eval_grid, S_COST))) return rc;
+  A.obs_w = c->obs_w.p; A.obs_flags = c->obs_flags.p; A.pt_fixed = c->pt_fixed.p;      // (prior rows: omvg_ba_debug_prior)
+  // the instantiation eval_jac launches for this scene
+  if ((rc = launch(c, c->has_ext ? eval_kernel<true, 4, true> : eval_kernel<true, 4, false>, c->eval_grid, EVAL_THREADS, 0, A)) ||
+      (rc = reduce_to(c, c->part.p, c->eval_grid, S_COST))) return rc;
   const long long n = c->no;
   std::vector<double> hr(2 * n), hp(6 * n), hc(12 * n), hi(2 * KI * n); double hcost = 0;
   OMVG_CUDA(cudaMemcpyAsync(hr.data(), c->r.p, hr.size() * 8, cudaMemcpyDeviceToHost, c->stream));
@@ -1176,6 +1178,26 @@ int omvg_ba_debug_eval(omvg_ba_ctx *c, const omvg_ba_options *O, double *cost, d
       if (J_intr) for (int k = 0; k < KI; ++k) J_intr[(o * 2 + row) * KI + k] = hi[(row * KI + k) * n + t];
     }
   }
+  return OMVG_OK;
+}
+
+int omvg_ba_debug_prior(omvg_ba_ctx *c, const omvg_ba_options *O, double *cost, double *r, double *J) {
+  if (!c || !O) return fail(OMVG_E_ARG, "null argument");
+  OMVG_CUDA(cudaSetDevice(c->device));
+  if (!c->npri) { if (cost) *cost = 0.0; return OMVG_OK; }
+  const Masks m = make_masks(c, O);
+  EvalArgs A; int rc = eval_prep(c, 0, A); if (rc) return rc;           // camR / camdR of the uploaded poses
+  PriorArgs PA{}; PA.poses = c->pose[0].p; PA.camR = c->camR[0].p; PA.camdR = c->camdR.p; PA.prior_pose = c->prior_pose.p; PA.center = c->prior_center.p; PA.weight = c->prior_weight.p;
+  PA.n = c->npri; PA.huber_a = c->prior_huber_a; PA.sc_cam = nullptr; PA.pose_mask = m.pose_mask; PA.rP = c->rP.p; PA.JP = c->JP.p; PA.cost_out = c->scal.p + S_COST;
+  if ((rc = launch(c, prior_eval_kernel<true>, 1, PRIOR_THREADS, 0, PA))) return rc;
+  std::vector<double> hr(3 * (size_t)c->npri), hJ(18 * (size_t)c->npri); double hcost = 0;
+  OMVG_CUDA(cudaMemcpyAsync(hr.data(), c->rP.p, hr.size() * 8, cudaMemcpyDeviceToHost, c->stream));
+  OMVG_CUDA(cudaMemcpyAsync(hJ.data(), c->JP.p, hJ.size() * 8, cudaMemcpyDeviceToHost, c->stream));
+  OMVG_CUDA(cudaMemcpyAsync(&hcost, c->scal.p + S_COST, 8, cudaMemcpyDeviceToHost, c->stream));
+  OMVG_CUDA(cudaStreamSynchronize(c->stream));
+  if (cost) *cost = hcost;
+  if (r) std::memcpy(r, hr.data(), hr.size() * 8);
+  if (J) std::memcpy(J, hJ.data(), hJ.size() * 8);
   return OMVG_OK;
 }
 

@@ -88,8 +88,10 @@ __device__ __forceinline__ bool inv3_spd(const double m[6], double inv[9]) {
 // ------------------------------------------------------------------------------ per-pose rotation
 // camR[p][9] row-major R(w); camdR[p][k][9] = dR/dw_k.  Same expression as AngleAxisRotatePoint:
 // R = cos I + sin [w]x + (1-cos) w w^T with w = aa/theta;  theta^2 <= eps: R = I + [aa]x.
-// camrec[p][22] = {R (9), Jr (9, row-major; column k = vee(R' dR_k), so dR_k X = R (Jr e_k x X)), t (3), pad}:
-// the compact per-pose record the per-observation kernel gathers with 11 x 16-byte loads.
+// camrec[p][22] = {R (9), Jr (9, row-major; column k = vee(R' dR_k), so dR_k X = R (Jr e_k x X)), t (3), taylor}:
+// the compact per-pose record the per-observation kernel gathers with 11 x 16-byte loads.  R' dR_k is skew only when
+// R is a rotation; the Taylor branch's R = I + [aa]x is not (R (j_k x X) would be off by O(|aa|)), so there Jr = I,
+// taylor = 1 and the evaluation takes dR_k X = e_k x X as it is.
 constexpr int CAMREC = 22;
 __global__ void cam_prep_kernel(const double *__restrict__ poses, int n_poses, double *__restrict__ camR, double *__restrict__ camdR, double *__restrict__ camrec) {
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
@@ -98,7 +100,8 @@ __global__ void cam_prep_kernel(const double *__restrict__ poses, int n_poses, d
   D aa[3]; for (int k = 0; k < 3; ++k) aa[k] = dvar<3>(poses[6 * p + k], k);
   const D theta2 = aa[0] * aa[0] + aa[1] * aa[1] + aa[2] * aa[2];
   D R[9];
-  if (theta2.a > DBL_EPSILON) {
+  const bool taylor = !(theta2.a > DBL_EPSILON);
+  if (!taylor) {
     const D theta = dsqrt(theta2), c = dcos(theta), s = dsin(theta), ti = dconst<3>(1.0) / theta;
     const D w[3] = {aa[0] * ti, aa[1] * ti, aa[2] * ti};
     const D omc = dconst<3>(1.0) - c;
@@ -122,9 +125,11 @@ __global__ void cam_prep_kernel(const double *__restrict__ poses, int n_poses, d
   for (int k = 0; k < 3; ++k) {
     double M[9];                                             // R' dR_k  (skew up to rounding)
     for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) { double v = 0; for (int l = 0; l < 3; ++l) v += R[l * 3 + i].a * R[l * 3 + j].v[k]; M[i * 3 + j] = v; }
-    rec[9 + 0 * 3 + k] = 0.5 * (M[7] - M[5]); rec[9 + 1 * 3 + k] = 0.5 * (M[2] - M[6]); rec[9 + 2 * 3 + k] = 0.5 * (M[3] - M[1]);
+    rec[9 + 0 * 3 + k] = taylor ? (k == 0) : 0.5 * (M[7] - M[5]);
+    rec[9 + 1 * 3 + k] = taylor ? (k == 1) : 0.5 * (M[2] - M[6]);
+    rec[9 + 2 * 3 + k] = taylor ? (k == 2) : 0.5 * (M[3] - M[1]);
   }
-  rec[18] = poses[6 * p + 3]; rec[19] = poses[6 * p + 4]; rec[20] = poses[6 * p + 5]; rec[21] = 0.0;
+  rec[18] = poses[6 * p + 3]; rec[19] = poses[6 * p + 4]; rec[20] = poses[6 * p + 5]; rec[21] = taylor ? 1.0 : 0.0;
 }
 
 // ------------------------------------------------------------------------------ problem setup on the device
@@ -393,14 +398,16 @@ __global__ void __launch_bounds__(EVAL_THREADS, MINB) eval_kernel(EvalArgs A) {
         __stcs(A.Jp + (1 * 3 + c) * n + o, sc * (g[3] * R[c] + g[4] * R[3 + c] + g[5] * R[6 + c]));
       }
       // pose block: rotation columns g * (dR_k X), translation columns g
+      // (read again here rather than kept from the gather above: holding R[21] live this far costs a spill)
+      const bool taylor = __ldg(A.camrec + (size_t)CAMREC * ip + 21) != 0.0;
       #pragma unroll
       for (int k = 0; k < 3; ++k) {
-        // dR_k X = R (j_k x X), j_k = column k of Jr
+        // dR_k X = R (j_k x X), j_k = column k of Jr;  Taylor branch: e_k x X (Jr = I)
         const double j0 = R[9 + k], j1 = R[12 + k], j2 = R[15 + k];
         const double v0 = j1 * X2 - j2 * X1, v1 = j2 * X0 - j0 * X2, v2 = j0 * X1 - j1 * X0;
-        const double q0 = R[0] * v0 + R[1] * v1 + R[2] * v2;
-        const double q1 = R[3] * v0 + R[4] * v1 + R[5] * v2;
-        const double q2 = R[6] * v0 + R[7] * v1 + R[8] * v2;
+        const double q0 = taylor ? v0 : R[0] * v0 + R[1] * v1 + R[2] * v2;
+        const double q1 = taylor ? v1 : R[3] * v0 + R[4] * v1 + R[5] * v2;
+        const double q2 = taylor ? v2 : R[6] * v0 + R[7] * v1 + R[8] * v2;
         const double sc = ((A.pose_mask >> k) & 1) ? (A.sc_cam ? A.sc_cam[6 * ip + k] : 1.0) : 0.0;
         __stcs(A.Jc + (0 * 6 + k) * n + o, sc * (g[0] * q0 + g[1] * q1 + g[2] * q2));
         __stcs(A.Jc + (1 * 6 + k) * n + o, sc * (g[3] * q0 + g[4] * q1 + g[5] * q2));
