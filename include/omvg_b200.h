@@ -201,6 +201,39 @@ int omvg_geom_essential_acransac(int device, uint64_t n_pairs, const uint64_t *o
 /* Validation aid (tests only): the device five-point solver on n independent samples of 5 bearing pairs.
  * b1, b2 [n][5][3]; out: E[n][10][9] (the first n_models[s] rows of sample s are its real solutions, row-major). */
 int omvg_geom_debug_five_point(int device, uint32_t n, const double *b1, const double *b2, double *E, int32_t *n_models);
+/* The angular essential-matrix models, for any calibrated camera (spherical included): GeometricFilter_ESphericalMatrix_AC_
+ * Angular<false | true>::Robust_estimation (matching_image_collection/E_ACRobust_Angular.hpp:52-160), i.e.
+ * ACKernelAdaptor_AngularRadianError<EightPointRelativePoseSolver (OMVG_GEOM_ESSENTIAL_ANGULAR, `-g a`) |
+ * ThreePointUprightRelativePoseSolver (OMVG_GEOM_ESSENTIAL_UPRIGHT, `-g u`), AngularError> + ACRANSAC on bearing vectors,
+ * then RelativePoseFromEssential (multiview/motion_from_essential.cpp:20-95) on the AC-RANSAC inliers.
+ *   bI, bJ [n_matches][3]     bearing vectors (*cam)(x) of the matched features of view I / J; finite
+ *   precision_deg             upper bound in degrees, as the functor takes it (main_GeometricFilter passes 4.0); finite
+ *                             and > 0, else OMVG_E_UNSUPPORTED.  ACRANSAC receives D2R(precision_deg) as its bound of the
+ *                             SQUARED angular residual, as the reference passes it.
+ * out: inliers / n_inliers   the list after the cheirality step (ascending match index; empty when
+ *                            RelativePoseFromEssential returns false); the reference keeps the pair iff n_inliers >
+ *                            2.5 * 8 (eight-point) or 2.5 * 3 (upright)
+ *      E[n_pairs][9]         row-major, the model ACRANSAC kept (identity when none)
+ *      stats[n_pairs][2]     {errorMax in radians, minNFA}
+ *      n_ransac_inliers      (nullable) the AC-RANSAC inlier count before the cheirality step
+ *      ransac_inliers        (nullable) [n_matches]: the AC-RANSAC list before the cheirality step (pair p: the first
+ *                            n_ransac_inliers[p] entries of its segment; needs n_ransac_inliers to be read)
+ * omvg_geom_acransac rejects both models: it takes pixel positions, not bearing vectors. */
+#define OMVG_GEOM_ESSENTIAL_ANGULAR 3
+#define OMVG_GEOM_ESSENTIAL_UPRIGHT 4
+int omvg_geom_angular_acransac(int device, int32_t model, uint64_t n_pairs, const uint64_t *offsets,
+                               const double *bI, const double *bJ, double precision_deg, uint32_t max_iterations,
+                               uint32_t *inliers, uint32_t *n_inliers, double *E, double *stats,
+                               uint32_t *n_ransac_inliers /* nullable */, uint32_t *ransac_inliers /* nullable */);
+/* Validation aids (tests only).  omvg_geom_debug_angular_solver: the device solver of `model` on n independent samples
+ * of 8 (eight-point) or 3 (upright) bearing pairs, b1, b2 [n][ms][3]; out E[n][9] row-major.
+ * omvg_geom_debug_relative_pose: RelativePoseFromEssential(b1, b2, E, index) as the filter runs it; out counts[4] (the
+ * cheirality count of each pose of MotionFromEssential, in the reference's pose order), selected[*n_selected] (the
+ * chosen pose's list, in the order of index) and *result (the function's boolean; false gives *n_selected = 0). */
+int omvg_geom_debug_angular_solver(int device, int32_t model, uint32_t n, const double *b1, const double *b2, double *E);
+int omvg_geom_debug_relative_pose(int device, const double *E, uint32_t n_bearings, const double *b1, const double *b2,
+                                  uint32_t n_index, const uint32_t *index, int32_t *counts, uint32_t *selected,
+                                  uint32_t *n_selected, int32_t *result);
 
 /* ===================================================================== BA ================= */
 #define OMVG_BA_INTR_STRIDE 8   /* doubles reserved per intrinsic block */

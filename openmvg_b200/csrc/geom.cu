@@ -1,5 +1,5 @@
-// geom.cu — per-pair a-contrario RANSAC (fundamental-matrix, homography and essential-matrix models) on sm_90a: the geometric filter openMVG runs
-// right after putative matching (SURVEY §8f N4).
+// geom.cu — per-pair a-contrario RANSAC (fundamental-matrix, homography, essential-matrix and angular essential-matrix models) on sm_90a: the
+// geometric filter openMVG runs right after putative matching (SURVEY §8f N4).
 //
 // Replaces (reference, $OPENMVG/src/openMVG):
 //   matching_image_collection/GeometricFilter.hpp:66-128          the pair loop (OpenMP over pairs)
@@ -749,6 +749,376 @@ __global__ void __launch_bounds__(THREADS) acransac_kernel(Args A) {
   }
 }
 
+// ---------------------------------------------------------------- angular essential models (DESIGN §3.10)
+// GeometricFilter_ESphericalMatrix_AC_Angular<UPRIGHT> (matching_image_collection/E_ACRobust_Angular.hpp:52-160):
+// ACKernelAdaptor_AngularRadianError<EightPointRelativePoseSolver | ThreePointUprightRelativePoseSolver, AngularError>
+// + ACRANSAC on bearing vectors, then RelativePoseFromEssential on the AC-RANSAC inliers.  A sibling of
+// acransac_kernel with its own arguments and shared memory, so the F/H and E instantiations are untouched.
+struct AngArgs {
+  const unsigned long long *offsets;       // [n_pairs + 1] into the match arrays
+  const double *bI, *bJ;                   // [n_matches][3] bearing vectors of view I / J
+  double max_threshold; unsigned int iterations;   // maxThreshold = D2R(precision) (squared radians), as ACRANSAC forms it
+  float *logc_n, *logc_k, *l10;            // scratch [n_matches + n_pairs] each
+  uint32_t *vec_index;                     // scratch [n_matches]
+  uint32_t *inliers;                       // out [n_matches]: the first n_inliers[p] entries of pair p's segment
+  uint32_t *n_inliers, *n_ransac;          // out [n_pairs]: after / before the cheirality step
+  uint32_t *ransac_inliers;                // out [n_matches] or null: the AC-RANSAC list before the cheirality step
+  double *E, *stats;                       // out [n_pairs][9], [n_pairs][2] = {errorMax (radians), minNFA}
+  unsigned int n_pairs;
+};
+
+struct SmemAng {
+  uint32_t mt[624];
+  double AtA[9][9], V[9][9], f1[9], f2[9], model[9];
+  double R[4][9], t[4][3];                 // the four poses of MotionFromEssential: rotation, translation()
+  int hist[NBINS]; int n_le; int warp_cnt[THREADS / 32];
+  int counts[4];
+  uint32_t sample[8];
+  int better_now, n_keep;
+  double nfa_thr, nfa_val;
+};
+
+// AngularError::Error (solver_essential_eight_point.cpp:50-60): |asin(x2 . normalize(E x1))|, with the FMAs the
+// reference's x86-64-v3 build forms (E x1: rows 0 and 1 as (E0 x0) + E1 x1 + E2 x2, row 2 as (E1 x1) + E2 x2 + E0 x0;
+// the last term of the squared norm and of the dot product fused).  E row-major.
+__device__ __forceinline__ double angular_error(const double *E, const double *a, const double *b) {
+  double m0 = __fma_rn(E[2], a[2], __fma_rn(E[1], a[1], E[0] * a[0]));
+  double m1 = __fma_rn(E[5], a[2], __fma_rn(E[4], a[1], E[3] * a[0]));
+  double m2 = __fma_rn(E[6], a[0], __fma_rn(E[8], a[2], E[7] * a[1]));
+  const double z = __fma_rn(m2, m2, m0 * m0 + m1 * m1);
+  if (z > 0.0) { const double s = sqrt(z); m0 /= s; m1 /= s; m2 /= s; }
+  return fabs(asin(__fma_rn(m2, b[2], b[0] * m0 + b[1] * m1)));
+}
+
+// cyclic Jacobi on a symmetric N x N (the same sweeps as smallest_two_eigvecs); A ends diagonal, V holds the vectors
+template <int N>
+__device__ void jacobi_sym(double (*A)[N], double (*V)[N]) {
+  for (int i = 0; i < N; ++i) for (int j = 0; j < N; ++j) V[i][j] = i == j ? 1.0 : 0.0;
+  for (int sweep = 0; sweep < 60; ++sweep) {
+    double off = 0, diag = 0;
+    for (int i = 0; i < N; ++i) { diag += A[i][i] * A[i][i]; for (int j = i + 1; j < N; ++j) off += A[i][j] * A[i][j]; }
+    if (off <= 1e-60 * diag || off == 0.0) break;
+    for (int p = 0; p < N - 1; ++p)
+      for (int q = p + 1; q < N; ++q) {
+        const double apq = A[p][q];
+        if (apq == 0.0) continue;
+        const double theta = (A[q][q] - A[p][p]) / (2.0 * apq);
+        const double t = (theta >= 0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+        for (int k = 0; k < N; ++k) { const double akp = A[k][p], akq = A[k][q]; A[k][p] = c * akp - s * akq; A[k][q] = s * akp + c * akq; }
+        for (int k = 0; k < N; ++k) { const double apk = A[p][k], aqk = A[q][k]; A[p][k] = c * apk - s * aqk; A[q][k] = s * apk + c * aqk; }
+        for (int k = 0; k < N; ++k) { const double vkp = V[k][p], vkq = V[k][q]; V[k][p] = c * vkp - s * vkq; V[k][q] = s * vkp + c * vkq; }
+      }
+  }
+}
+
+// EightPointRelativePoseSolver::Solve (solver_essential_eight_point.cpp:15-46; the closest-essential projection runs
+// only for more than 8 rows, never here) or ThreePointUprightRelativePoseSolver::Solve (solver_essential_three_point.cpp:
+// 86-114).  A'A summed in sample order, one entry per thread; thread 0 runs Jacobi.  Called by the whole block; S.model out.
+template <bool UPRIGHT>
+__device__ void angular_solve(SmemAng &S, const double *b1, const double *b2, const uint32_t *sample) {
+  if (UPRIGHT) {
+    if (threadIdx.x < 16) {
+      const int i = threadIdx.x / 4, j = threadIdx.x % 4;
+      double acc = 0;
+      for (int t = 0; t < 3; ++t) {
+        const double *a = b1 + 3 * (size_t)sample[t], *b = b2 + 3 * (size_t)sample[t];
+        const double r[4] = {a[0] * b[1], -a[2] * b[1], -b[0] * a[1], -b[2] * a[1]};
+        acc += r[i] * r[j];
+      }
+      S.AtA[i][j] = acc;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      double A4[4][4], V4[4][4];
+      for (int i = 0; i < 4; ++i) for (int j = 0; j < 4; ++j) A4[i][j] = S.AtA[i][j];
+      jacobi_sym<4>(A4, V4);
+      int k = 0; for (int i = 1; i < 4; ++i) if (A4[i][i] < A4[k][k]) k = i;
+      for (int i = 0; i < 9; ++i) S.model[i] = 0.0;
+      S.model[1] = V4[2][k]; S.model[3] = -V4[0][k]; S.model[5] = V4[1][k]; S.model[7] = V4[3][k];
+    }
+  } else {
+    if (threadIdx.x < 81) {                                        // EncodeEpipolarEquation: row = x2(k) * x1'
+      const int i = threadIdx.x / 9, j = threadIdx.x % 9;
+      double acc = 0;
+      for (int t = 0; t < 8; ++t) {
+        const size_t s = sample[t];
+        acc += (b2[3 * s + i / 3] * b1[3 * s + i % 3]) * (b2[3 * s + j / 3] * b1[3 * s + j % 3]);
+      }
+      S.AtA[i][j] = acc;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      smallest_two_eigvecs(S.AtA, S.V, S.f1, S.f2);
+      for (int i = 0; i < 9; ++i) S.model[i] = S.f1[i];
+    }
+  }
+  __syncthreads();
+}
+
+// MotionFromEssential (multiview/essential.cpp:79-113).  The SVD is formed from the Jacobi eigenvectors of E'E
+// (descending): u_i = E v_i / |E v_i| for the two largest, u_3 = u_1 x u_2; then the reference's determinant fix-ups.
+// Poses in the reference's order {(R0, t0), (R1, t1), (R0, t1), (R1, t0)}, each restated as Pose3(R, -R' t).translation().
+__device__ void motion_from_essential(const double *E, double (*R)[9], double (*t)[3]) {
+  double M[3][3], V[3][3];
+  for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) { double v = 0; for (int k = 0; k < 3; ++k) v += E[3 * k + i] * E[3 * k + j]; M[i][j] = v; }
+  jacobi_sym<3>(M, V);
+  int o[3] = {0, 1, 2};
+  for (int a = 0; a < 2; ++a) for (int b = 0; b < 2 - a; ++b) if (M[o[b + 1]][o[b + 1]] > M[o[b]][o[b]]) { const int x = o[b]; o[b] = o[b + 1]; o[b + 1] = x; }
+  double U[3][3], Vt[3][3];
+  for (int c = 0; c < 3; ++c) for (int k = 0; k < 3; ++k) Vt[c][k] = V[k][o[c]];
+  for (int c = 0; c < 2; ++c) {
+    double u[3], n2 = 0;
+    for (int r = 0; r < 3; ++r) { u[r] = E[3 * r] * Vt[c][0] + E[3 * r + 1] * Vt[c][1] + E[3 * r + 2] * Vt[c][2]; n2 += u[r] * u[r]; }
+    const double n = sqrt(n2);
+    for (int r = 0; r < 3; ++r) U[r][c] = u[r] / n;
+  }
+  U[0][2] = U[1][0] * U[2][1] - U[2][0] * U[1][1];
+  U[1][2] = U[2][0] * U[0][1] - U[0][0] * U[2][1];
+  U[2][2] = U[0][0] * U[1][1] - U[1][0] * U[0][1];
+  auto det3 = [](const double (*m)[3]) {
+    return m[0][0] * (m[1][1] * m[2][2] - m[1][2] * m[2][1]) - m[0][1] * (m[1][0] * m[2][2] - m[1][2] * m[2][0]) + m[0][2] * (m[1][0] * m[2][1] - m[1][1] * m[2][0]);
+  };
+  if (det3(U) < 0) for (int r = 0; r < 3; ++r) U[r][2] = -U[r][2];
+  if (det3(Vt) < 0) for (int k = 0; k < 3; ++k) Vt[2][k] = -Vt[2][k];
+  const double W[2][3][3] = {{{0, -1, 0}, {1, 0, 0}, {0, 0, 1}}, {{0, 1, 0}, {-1, 0, 0}, {0, 0, 1}}};
+  double Rw[2][9];
+  for (int w = 0; w < 2; ++w) {
+    double T[3][3];
+    for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) { double v = 0; for (int k = 0; k < 3; ++k) v += U[r][k] * W[w][k][c]; T[r][c] = v; }
+    for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) { double v = 0; for (int k = 0; k < 3; ++k) v += T[r][k] * Vt[k][c]; Rw[w][3 * r + c] = v; }
+  }
+  const int PR[4] = {0, 1, 0, 1}, PT[4] = {0, 1, 1, 0};
+  for (int p = 0; p < 4; ++p) {
+    const double *Rp = Rw[PR[p]];
+    const double s = PT[p] ? -1.0 : 1.0;
+    const double tp[3] = {s * U[0][2], s * U[1][2], s * U[2][2]};
+    double C[3];
+    for (int i = 0; i < 3; ++i) { double v = 0; for (int k = 0; k < 3; ++k) v += -Rp[3 * k + i] * tp[k]; C[i] = v; }
+    for (int i = 0; i < 3; ++i) { double v = 0; for (int k = 0; k < 3; ++k) v += Rp[3 * i + k] * C[k]; t[p][i] = -v; }
+    for (int i = 0; i < 9; ++i) R[p][i] = Rp[i];
+  }
+}
+
+// TriangulateIDWMidpoint (multiview/triangulation.cpp:179-216) between (I, 0) and (R, t): the Eq. (9) cheirality test
+// only.  NaN norms (parallel rays) make every comparison false, as in the reference.
+__device__ __forceinline__ bool idw_midpoint_cheirality(const double *R, const double *t, const double *x0, const double *x1) {
+  double Rx0[3];
+  for (int i = 0; i < 3; ++i) Rx0[i] = R[3 * i] * x0[0] + R[3 * i + 1] * x0[1] + R[3 * i + 2] * x0[2];
+  auto norm_cross = [](const double *a, const double *b) {
+    const double c0 = a[1] * b[2] - a[2] * b[1], c1 = a[2] * b[0] - a[0] * b[2], c2 = a[0] * b[1] - a[1] * b[0];
+    return sqrt(c0 * c0 + c1 * c1 + c2 * c2);
+  };
+  const double p = norm_cross(Rx0, x1), q = norm_cross(Rx0, t), r = norm_cross(x1, t);
+  const double l0 = r / p, l1 = q / p;
+  double e[4] = {0, 0, 0, 0};                                      // t + l0 Rx0 -+ l1 x1, t - l0 Rx0 -+ l1 x1
+  for (int i = 0; i < 3; ++i) {
+    const double a = l0 * Rx0[i], b = l1 * x1[i];
+    const double v0 = t[i] + a - b, v1 = t[i] + a + b, v2 = t[i] - a - b, v3 = t[i] - a + b;
+    e[0] += v0 * v0; e[1] += v1 * v1; e[2] += v2 * v2; e[3] += v3 * v3;
+  }
+  // The reference takes std::min (vminsd), which fmin differs from only when an operand is NaN.  All four sums come from
+  // the same l0, l1, t, Rx0, x1: a NaN in e[1..3] means a NaN l0 or l1, which makes e[0] NaN too, and then both forms
+  // compare false.  With e[0] finite the two minima are equal.
+  return e[0] < fmin(fmin(e[1], e[2]), e[3]);
+}
+
+// RelativePoseFromEssential (multiview/motion_from_essential.cpp:20-95) over idx[0..n), called by the whole block.  On
+// true, idx[0..returned) is compacted in place to the chosen pose's list (ascending, as given); on false 0 is returned.
+// S.counts holds the four cheirality counts afterwards.
+__device__ unsigned int relative_pose_from_essential(SmemAng &S, const double *E, const double *b1, const double *b2,
+                                                     uint32_t *idx, unsigned int n) {
+  if (threadIdx.x == 0) motion_from_essential(E, S.R, S.t);
+  if (threadIdx.x < 4) S.counts[threadIdx.x] = 0;
+  __syncthreads();
+  int c[4] = {0, 0, 0, 0};
+  for (unsigned int k = threadIdx.x; k < n; k += THREADS) {
+    const size_t i = idx[k];
+    for (int p = 0; p < 4; ++p) c[p] += idw_midpoint_cheirality(S.R[p], S.t[p], b1 + 3 * i, b2 + 3 * i);
+  }
+  for (int p = 0; p < 4; ++p) {
+    for (int o = 16; o > 0; o >>= 1) c[p] += __shfl_xor_sync(0xffffffffu, c[p], o);
+    if ((threadIdx.x & 31) == 0) atomicAdd(&S.counts[p], c[p]);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int best = 0; for (int p = 1; p < 4; ++p) if (S.counts[p] > S.counts[best]) best = p;   // the first maximal count
+    int second = -1; for (int p = 0; p < 4; ++p) if (p != best && S.counts[p] > second) second = S.counts[p];
+    const bool ok = S.counts[best] > 0 && second / (double)S.counts[best] < 0.7;
+    S.n_keep = ok ? best : -1;
+  }
+  __syncthreads();
+  const int best = S.n_keep;
+  if (best < 0) return 0;
+  unsigned int base = 0;
+  for (unsigned int k0 = 0; k0 < n; k0 += THREADS) {                // ordered in-place compaction
+    const unsigned int k = k0 + threadIdx.x;
+    uint32_t i = 0; bool in = false;
+    if (k < n) { i = idx[k]; in = idw_midpoint_cheirality(S.R[best], S.t[best], b1 + 3 * (size_t)i, b2 + 3 * (size_t)i); }
+    const unsigned int bal = __ballot_sync(0xffffffffu, in);
+    if ((threadIdx.x & 31) == 0) S.warp_cnt[threadIdx.x >> 5] = __popc(bal);
+    __syncthreads();
+    unsigned int pre = base;
+    for (int w = 0; w < (int)(threadIdx.x >> 5); ++w) pre += S.warp_cnt[w];
+    if (in) idx[pre + __popc(bal & ((1u << (threadIdx.x & 31)) - 1u))] = i;
+    unsigned int tot = 0; for (int w = 0; w < THREADS / 32; ++w) tot += S.warp_cnt[w];
+    base += tot;
+    __syncthreads();
+  }
+  return base;
+}
+
+template <bool UPRIGHT>
+__global__ void __launch_bounds__(THREADS) angular_acransac_kernel(AngArgs A) {
+  __shared__ SmemAng S;
+  const double INF = __longlong_as_double(0x7ff0000000000000ll);
+  constexpr int ms = UPRIGHT ? 3 : 8;                             // MINIMUM_SAMPLES; MAX_MODELS = 1
+  for (unsigned int pair = blockIdx.x; pair < A.n_pairs; pair += gridDim.x) {
+    __syncthreads();
+    const unsigned long long off = A.offsets[pair];
+    const unsigned int nData = (unsigned int)(A.offsets[pair + 1] - off);
+    const double *b1 = A.bI + 3 * off, *b2 = A.bJ + 3 * off;
+    uint32_t *vec_index = A.vec_index + off, *inl = A.inliers + off;
+    float *logc_n = A.logc_n + off + pair, *logc_k = A.logc_k + off + pair, *l10 = A.l10 + off + pair;
+    if (threadIdx.x == 0) {
+      A.n_inliers[pair] = 0; A.n_ransac[pair] = 0; A.stats[2 * pair] = 0.0; A.stats[2 * pair + 1] = 0.0;
+      for (int i = 0; i < 9; ++i) A.E[9 * (size_t)pair + i] = (i % 4 == 0) ? 1.0 : 0.0;
+    }
+    if (nData <= (unsigned int)ms) continue;                      // ACRANSAC: {0, 0}; RelativePoseFromEssential on no inliers: false
+    for (unsigned int i = threadIdx.x; i < nData; i += THREADS) vec_index[i] = i;
+    // ACKernelAdaptor_AngularRadianError: no normalisation, logalpha0 = log10(1/2), multError = 1/4
+    const double logalpha0 = log10(1. / 2.), mult_error = 1. / 4., maxThreshold = A.max_threshold;
+    for (unsigned int i = threadIdx.x; i <= nData; i += THREADS) l10[i] = (float)log10((double)(float)i);
+    __syncthreads();
+    for (unsigned int k = threadIdx.x; k <= nData; k += THREADS) {
+      { unsigned int kk = k; float r = 0.f;
+        if (kk < nData) { if (nData - kk < kk) kk = nData - kk; for (unsigned int i = 1; i <= kk; ++i) r += l10[nData - i + 1] - l10[i]; }
+        logc_n[k] = r; }
+      { unsigned int kk = (unsigned int)ms; const unsigned int m = k; float r = 0.f;
+        if (kk < m) { if (m - kk < kk) kk = m - kk; for (unsigned int i = 1; i <= kk; ++i) r += l10[m - i + 1] - l10[i]; }
+        logc_k[k] = r; }
+    }
+    const double loge0 = log10((double)1 * (double)(nData - ms));
+    __syncthreads();
+    Rng g{S.mt, 624};
+    if (threadIdx.x == 0) rng_seed(g, 5489u);
+    double minNFA = INF, errorMax = INF;
+    int nIterReserve = (int)(A.iterations / 10);
+    unsigned int nIter = A.iterations - nIterReserve;
+    bool bACRansacMode = false;
+    unsigned int n_inl = 0, index_size = nData;
+    for (unsigned int iter = 0; iter < nIter && iter < A.iterations; ++iter) {
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        if (bACRansacMode) sample_shuffle(g, ms, vec_index, index_size, S.sample); else sample_reject(g, ms, nData, S.sample);
+      }
+      __syncthreads();
+      angular_solve<UPRIGHT>(S, b1, b2, S.sample);
+      bool better = false;
+      if (threadIdx.x < NBINS) S.hist[threadIdx.x] = 0;
+      if (threadIdx.x == 0) { S.n_le = 0; S.better_now = 0; }
+      __syncthreads();
+      const double by_interval = NBINS / (maxThreshold - 0.0);
+      int le = 0;
+      for (unsigned int i = threadIdx.x; i < nData; i += THREADS) {
+        const double a = angular_error(S.model, b1 + 3 * (size_t)i, b2 + 3 * (size_t)i), e = a * a;
+        if (e <= maxThreshold) ++le;
+        if (e >= 0.0) { const unsigned long long b = (unsigned long long)((e - 0.0) * by_interval); if (b < (unsigned long long)NBINS) atomicAdd(&S.hist[(int)b], 1); }
+      }
+      if (!bACRansacMode) { for (int o = 16; o > 0; o >>= 1) le += __shfl_xor_sync(0xffffffffu, le, o); if ((threadIdx.x & 31) == 0) atomicAdd(&S.n_le, le); }
+      __syncthreads();
+      if (!bACRansacMode && (double)S.n_le > 2.5 * ms) bACRansacMode = true;
+      if (bACRansacMode) {
+        if (threadIdx.x == 0) {
+          const double feps = (double)FLT_EPSILON;
+          const double val = (maxThreshold - 0.0) / (double)(NBINS - 1);
+          double best_nfa = INF, best_thr = 0.0;
+          unsigned int cum = 0;
+          for (int bin = 0; bin < NBINS; ++bin) {
+            cum += (unsigned int)S.hist[bin];
+            const double rv = val * (double)bin + 0.0;
+            if (cum > (unsigned int)ms && rv > feps) {
+              const double logalpha = logalpha0 + mult_error * log10(rv + feps);
+              const double cur = loge0 + logalpha * (double)(cum - ms) + logc_n[cum] + logc_k[cum];
+              if (cur < best_nfa && cur < 0) { best_nfa = cur; best_thr = rv; }
+            }
+          }
+          if (best_nfa < minNFA) { S.better_now = 1; S.nfa_thr = best_thr; S.nfa_val = best_nfa; }
+        }
+        __syncthreads();
+        if (S.better_now) {
+          const double thr = S.nfa_thr;
+          unsigned int base = 0;
+          for (unsigned int i0 = 0; i0 < nData; i0 += THREADS) {
+            const unsigned int i = i0 + threadIdx.x;
+            bool in = false;
+            if (i < nData) { const double a = angular_error(S.model, b1 + 3 * (size_t)i, b2 + 3 * (size_t)i); in = a * a <= thr; }
+            const unsigned int bal = __ballot_sync(0xffffffffu, in);
+            if ((threadIdx.x & 31) == 0) S.warp_cnt[threadIdx.x >> 5] = __popc(bal);
+            __syncthreads();
+            unsigned int pre = base;
+            for (int w = 0; w < (int)(threadIdx.x >> 5); ++w) pre += S.warp_cnt[w];
+            if (in) inl[pre + __popc(bal & ((1u << (threadIdx.x & 31)) - 1u))] = i;
+            unsigned int tot = 0; for (int w = 0; w < THREADS / 32; ++w) tot += S.warp_cnt[w];
+            base += tot;
+            __syncthreads();
+          }
+          n_inl = base;
+          if (n_inl > (unsigned int)ms) {
+            better = true; minNFA = S.nfa_val; errorMax = thr;
+            if (threadIdx.x < 9) A.E[9 * (size_t)pair + threadIdx.x] = S.model[threadIdx.x];
+          }
+        }
+      }
+      __syncthreads();
+      if (!bACRansacMode && (int)iter > nIterReserve * 2) { nIter = 0; continue; }
+      if (bACRansacMode && ((better && minNFA < 0) || ((iter + 1) == nIter && nIterReserve > 0))) {
+        if (n_inl == 0) { ++nIter; --nIterReserve; }
+        else {
+          for (unsigned int i = threadIdx.x; i < n_inl; i += THREADS) vec_index[i] = inl[i];
+          index_size = n_inl;
+          if (nIterReserve) { nIter = iter + 1 + nIterReserve; nIterReserve = 0; }
+        }
+      }
+    }
+    __syncthreads();
+    if (minNFA >= 0) n_inl = 0;
+    if (threadIdx.x == 0) {
+      A.n_ransac[pair] = n_inl;
+      if (n_inl > 0) errorMax = sqrt(errorMax);                    // unormalizeError
+      A.stats[2 * pair] = errorMax; A.stats[2 * pair + 1] = minNFA;
+      for (int i = 0; i < 9; ++i) S.model[i] = A.E[9 * (size_t)pair + i];
+    }
+    if (A.ransac_inliers) for (unsigned int i = threadIdx.x; i < n_inl; i += THREADS) A.ransac_inliers[off + i] = inl[i];
+    __syncthreads();
+    const unsigned int n_final = relative_pose_from_essential(S, S.model, b1, b2, inl, n_inl);
+    if (threadIdx.x == 0) A.n_inliers[pair] = n_final;
+  }
+}
+
+// validation aids: one block per sample of ms bearing pairs / one RelativePoseFromEssential call
+template <bool UPRIGHT>
+__global__ void __launch_bounds__(THREADS) angular_solver_kernel(unsigned int n, const double *b1, const double *b2, double *E) {
+  __shared__ SmemAng S;
+  constexpr int ms = UPRIGHT ? 3 : 8;
+  if (threadIdx.x < ms) S.sample[threadIdx.x] = threadIdx.x;
+  for (unsigned int s = blockIdx.x; s < n; s += gridDim.x) {
+    __syncthreads();
+    angular_solve<UPRIGHT>(S, b1 + 3 * ms * (size_t)s, b2 + 3 * ms * (size_t)s, S.sample);
+    if (threadIdx.x < 9) E[9 * (size_t)s + threadIdx.x] = S.model[threadIdx.x];
+  }
+}
+
+__global__ void __launch_bounds__(THREADS) relative_pose_kernel(const double *E, const double *b1, const double *b2, uint32_t *idx,
+                                                                unsigned int n, int *counts, unsigned int *n_out) {
+  __shared__ SmemAng S;
+  if (threadIdx.x < 9) S.model[threadIdx.x] = E[threadIdx.x];
+  __syncthreads();
+  const unsigned int k = relative_pose_from_essential(S, S.model, b1, b2, idx, n);
+  if (threadIdx.x < 4) counts[threadIdx.x] = S.counts[threadIdx.x];
+  if (threadIdx.x == 0) *n_out = k;                                // 0: false (true keeps at least the best count > 0)
+}
+
 }}  // namespace omvg::geom
 
 namespace {
@@ -844,6 +1214,115 @@ extern "C" int omvg_geom_debug_five_point(int device, uint32_t n, const double *
   geom::five_point_kernel<<<std::min<uint32_t>(n, 64u * n_sms), 32>>>(n, d_b1.p, d_b2.p, d_E.p, d_n.p);
   OMVG_CUDA(cudaGetLastError());
   OMVG_CUDA(cudaMemcpy(E, d_E.p, n * 720ull, cudaMemcpyDeviceToHost)); OMVG_CUDA(cudaMemcpy(n_models, d_n.p, n * 4ull, cudaMemcpyDeviceToHost));
+  return OMVG_OK;
+}
+
+namespace {
+
+int check_bearings(const double *b, uint64_t n) {
+  for (uint64_t i = 0; i < 3 * n; ++i) if (!std::isfinite(b[i])) return omvg::fail(OMVG_E_ARG, "non-finite bearing vector %llu", (unsigned long long)(i / 3));
+  return OMVG_OK;
+}
+
+}  // namespace
+
+extern "C" int omvg_geom_angular_acransac(int device, int32_t model, uint64_t n_pairs, const uint64_t *offsets,
+                                          const double *bI, const double *bJ, double precision_deg, uint32_t max_iterations,
+                                          uint32_t *inliers, uint32_t *n_inliers, double *E, double *stats, uint32_t *n_ransac_inliers,
+                                          uint32_t *ransac_inliers) {
+  using namespace omvg;
+  if (model != OMVG_GEOM_ESSENTIAL_ANGULAR && model != OMVG_GEOM_ESSENTIAL_UPRIGHT) return fail(OMVG_E_ARG, "model %d is not an angular essential model (3 = eight-point, 4 = upright three-point)", model);
+  if (n_pairs && (!offsets || !n_inliers || !E || !stats)) return fail(OMVG_E_ARG, "null argument");
+  if (!(precision_deg > 0.0) || !std::isfinite(precision_deg)) return fail(OMVG_E_UNSUPPORTED, "the GPU filter needs a finite upper bound of the precision (main_GeometricFilter uses 4.0)");
+  if (max_iterations < 1) return fail(OMVG_E_ARG, "max_iterations must be >= 1");
+  int n_sms = 0;
+  if (const int rc = check_device(device, &n_sms)) return rc;
+  if (!n_pairs) return OMVG_OK;
+  for (uint64_t p = 0; p < n_pairs; ++p) if (offsets[p + 1] < offsets[p]) return fail(OMVG_E_ARG, "offsets must be non-decreasing");
+  const uint64_t nm = offsets[n_pairs];
+  if (nm && (!bI || !bJ || !inliers)) return fail(OMVG_E_ARG, "null match arrays");
+  if (nm >= (1ull << 31)) return fail(OMVG_E_UNSUPPORTED, "more than 2^31 putative matches in one call");
+  if (const int rc = check_bearings(bI, nm)) return rc;
+  if (const int rc = check_bearings(bJ, nm)) return rc;
+  OMVG_CUDA(cudaSetDevice(device));
+  struct Call { cudaStream_t stream = nullptr; long long launches = 0; ~Call() { if (stream) cudaStreamDestroy(stream); } } call;
+  OMVG_CUDA(cudaStreamCreateWithFlags(&call.stream, cudaStreamNonBlocking));
+  const cudaStream_t st = call.stream;
+  const size_t m1 = std::max<uint64_t>(nm, 1);
+  DevBuf<unsigned long long> d_off; DevBuf<double> d_bI, d_bJ, d_E, d_stats;
+  DevBuf<float> d_ln, d_lk, d_l10; DevBuf<uint32_t> d_idx, d_inl, d_ninl, d_nr, d_rinl;
+  if (d_off.alloc(n_pairs + 1) || d_bI.alloc(3 * m1) || d_bJ.alloc(3 * m1) || d_ln.alloc(nm + n_pairs) || d_lk.alloc(nm + n_pairs) ||
+      d_l10.alloc(nm + n_pairs) || d_idx.alloc(m1) || d_inl.alloc(m1) || d_ninl.alloc(n_pairs) || d_nr.alloc(n_pairs) ||
+      d_E.alloc(9 * n_pairs) || d_stats.alloc(2 * n_pairs) || (ransac_inliers && d_rinl.alloc(m1)))
+    return fail(OMVG_E_CUDA, "out of device memory");
+  OMVG_CUDA(cudaMemcpyAsync(d_off.p, offsets, (n_pairs + 1) * 8, cudaMemcpyHostToDevice, st));
+  if (nm) { OMVG_CUDA(cudaMemcpyAsync(d_bI.p, bI, nm * 24, cudaMemcpyHostToDevice, st)); OMVG_CUDA(cudaMemcpyAsync(d_bJ.p, bJ, nm * 24, cudaMemcpyHostToDevice, st)); }
+  geom::AngArgs A{};
+  A.offsets = d_off.p; A.bI = d_bI.p; A.bJ = d_bJ.p;
+  A.max_threshold = precision_deg * M_PI / 180.0;        // D2R (numeric.h:123-126); ACRANSAC takes it as the squared-error bound
+  A.iterations = max_iterations;
+  A.logc_n = d_ln.p; A.logc_k = d_lk.p; A.l10 = d_l10.p; A.vec_index = d_idx.p; A.inliers = d_inl.p;
+  A.n_inliers = d_ninl.p; A.n_ransac = d_nr.p; A.ransac_inliers = ransac_inliers ? d_rinl.p : nullptr; A.E = d_E.p; A.stats = d_stats.p; A.n_pairs = (unsigned int)n_pairs;
+  void (*kernel)(geom::AngArgs) = model == OMVG_GEOM_ESSENTIAL_UPRIGHT ? geom::angular_acransac_kernel<true> : geom::angular_acransac_kernel<false>;
+  int per_sm = 1; OMVG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, geom::THREADS, 0));
+  const unsigned int grid = (unsigned int)std::min<uint64_t>(n_pairs, (uint64_t)n_sms * std::max(1, per_sm));
+  if (const int rc = launch(&call, kernel, grid, geom::THREADS, 0, A)) return rc;
+  if (nm) OMVG_CUDA(cudaMemcpyAsync(inliers, d_inl.p, nm * 4, cudaMemcpyDeviceToHost, st));
+  OMVG_CUDA(cudaMemcpyAsync(n_inliers, d_ninl.p, n_pairs * 4, cudaMemcpyDeviceToHost, st));
+  if (n_ransac_inliers) OMVG_CUDA(cudaMemcpyAsync(n_ransac_inliers, d_nr.p, n_pairs * 4, cudaMemcpyDeviceToHost, st));
+  if (ransac_inliers && nm) OMVG_CUDA(cudaMemcpyAsync(ransac_inliers, d_rinl.p, nm * 4, cudaMemcpyDeviceToHost, st));
+  OMVG_CUDA(cudaMemcpyAsync(E, d_E.p, n_pairs * 72, cudaMemcpyDeviceToHost, st));
+  OMVG_CUDA(cudaMemcpyAsync(stats, d_stats.p, n_pairs * 16, cudaMemcpyDeviceToHost, st));
+  OMVG_CUDA(cudaStreamSynchronize(st));
+  return OMVG_OK;
+}
+
+extern "C" int omvg_geom_debug_angular_solver(int device, int32_t model, uint32_t n, const double *b1, const double *b2, double *E) {
+  using namespace omvg;
+  if (model != OMVG_GEOM_ESSENTIAL_ANGULAR && model != OMVG_GEOM_ESSENTIAL_UPRIGHT) return fail(OMVG_E_ARG, "model %d is not an angular essential model", model);
+  if (n && (!b1 || !b2 || !E)) return fail(OMVG_E_ARG, "null argument");
+  int n_sms = 0;
+  if (const int rc = check_device(device, &n_sms)) return rc;
+  if (!n) return OMVG_OK;
+  const size_t ms = model == OMVG_GEOM_ESSENTIAL_UPRIGHT ? 3 : 8;
+  OMVG_CUDA(cudaSetDevice(device));
+  DevBuf<double, CudaAlloc> d_b1, d_b2, d_E;
+  int rc;
+  if ((rc = d_b1.alloc(3 * ms * n)) || (rc = d_b2.alloc(3 * ms * n)) || (rc = d_E.alloc(9ull * n))) return rc;
+  OMVG_CUDA(cudaMemcpy(d_b1.p, b1, 24 * ms * n, cudaMemcpyHostToDevice)); OMVG_CUDA(cudaMemcpy(d_b2.p, b2, 24 * ms * n, cudaMemcpyHostToDevice));
+  const unsigned int grid = std::min<uint32_t>(n, 16u * n_sms);
+  if (model == OMVG_GEOM_ESSENTIAL_UPRIGHT) geom::angular_solver_kernel<true><<<grid, geom::THREADS>>>(n, d_b1.p, d_b2.p, d_E.p);
+  else geom::angular_solver_kernel<false><<<grid, geom::THREADS>>>(n, d_b1.p, d_b2.p, d_E.p);
+  OMVG_CUDA(cudaGetLastError());
+  OMVG_CUDA(cudaMemcpy(E, d_E.p, n * 72ull, cudaMemcpyDeviceToHost));
+  return OMVG_OK;
+}
+
+extern "C" int omvg_geom_debug_relative_pose(int device, const double *E, uint32_t n_bearings, const double *b1, const double *b2,
+                                             uint32_t n_index, const uint32_t *index, int32_t *counts, uint32_t *selected,
+                                             uint32_t *n_selected, int32_t *result) {
+  using namespace omvg;
+  if (!E || !counts || !n_selected || !result || (n_bearings && (!b1 || !b2)) || (n_index && (!index || !selected))) return fail(OMVG_E_ARG, "null argument");
+  for (int i = 0; i < 9; ++i) if (!std::isfinite(E[i])) return fail(OMVG_E_ARG, "non-finite E");
+  for (uint32_t k = 0; k < n_index; ++k) if (index[k] >= n_bearings) return fail(OMVG_E_ARG, "index %u out of range", k);
+  if (const int rc = check_bearings(b1, n_bearings)) return rc;
+  if (const int rc = check_bearings(b2, n_bearings)) return rc;
+  int n_sms = 0;
+  if (const int rc = check_device(device, &n_sms)) return rc;
+  OMVG_CUDA(cudaSetDevice(device));
+  DevBuf<double, CudaAlloc> d_E, d_b1, d_b2; DevBuf<uint32_t, CudaAlloc> d_idx, d_n; DevBuf<int, CudaAlloc> d_c;
+  int rc;
+  if ((rc = d_E.alloc(9)) || (rc = d_b1.alloc(3ull * std::max(n_bearings, 1u))) || (rc = d_b2.alloc(3ull * std::max(n_bearings, 1u))) ||
+      (rc = d_idx.alloc(std::max(n_index, 1u))) || (rc = d_n.alloc(1)) || (rc = d_c.alloc(4))) return rc;
+  OMVG_CUDA(cudaMemcpy(d_E.p, E, 72, cudaMemcpyHostToDevice));
+  if (n_bearings) { OMVG_CUDA(cudaMemcpy(d_b1.p, b1, 24ull * n_bearings, cudaMemcpyHostToDevice)); OMVG_CUDA(cudaMemcpy(d_b2.p, b2, 24ull * n_bearings, cudaMemcpyHostToDevice)); }
+  if (n_index) OMVG_CUDA(cudaMemcpy(d_idx.p, index, 4ull * n_index, cudaMemcpyHostToDevice));
+  geom::relative_pose_kernel<<<1, geom::THREADS>>>(d_E.p, d_b1.p, d_b2.p, d_idx.p, n_index, d_c.p, d_n.p);
+  OMVG_CUDA(cudaGetLastError());
+  OMVG_CUDA(cudaMemcpy(counts, d_c.p, 16, cudaMemcpyDeviceToHost));
+  OMVG_CUDA(cudaMemcpy(n_selected, d_n.p, 4, cudaMemcpyDeviceToHost));
+  if (*n_selected) OMVG_CUDA(cudaMemcpy(selected, d_idx.p, 4ull * *n_selected, cudaMemcpyDeviceToHost));
+  *result = *n_selected > 0;
   return OMVG_OK;
 }
 

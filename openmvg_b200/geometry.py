@@ -73,3 +73,57 @@ def debug_five_point(b1, b2, device: int = 0):
     p = lambda a: a.ctypes.data_as(_vp)   # noqa: E731
     check(lib().omvg_geom_debug_five_point(int(device), ctypes.c_uint32(n), p(b1), p(b2), p(E), p(k)))
     return dict(E=E[:n].reshape(n, 10, 3, 3).copy(), n_models=k[:n].copy())
+
+
+ESSENTIAL_ANGULAR, ESSENTIAL_UPRIGHT = 3, 4
+
+
+def angular_essential_acransac(offsets, bI, bJ, upright: bool = False, precision_deg: float = 4.0, max_iterations: int = 2048,
+                               device: int = 0):
+    """GeometricFilter_ESphericalMatrix_AC_Angular<upright>::Robust_estimation per pair (E_ACRobust_Angular.hpp:52-160)
+    over a CSR of putative matches given as bearing vectors bI, bJ [n_matches, 3] ((*cam)(x) of each view).  Eight-point
+    (`-g a`) or, with upright=True, upright three-point (`-g u`) AC-RANSAC, then RelativePoseFromEssential.
+    -> list of dicts per pair: inliers (after the cheirality step: what the filter keeps), ransac_inliers (the AC-RANSAC
+    list before it), F [3,3] (holds E), error_max (radians), min_nfa.  The reference keeps a pair iff it has more than
+    20 (eight-point) or 7.5 (upright) inliers."""
+    off = np.ascontiguousarray(offsets, np.uint64); n_pairs = len(off) - 1
+    bI = np.ascontiguousarray(bI, np.float64).reshape(-1, 3); bJ = np.ascontiguousarray(bJ, np.float64).reshape(-1, 3)
+    nm = int(off[-1]); assert len(bI) == nm == len(bJ)
+    inl = np.zeros(max(nm, 1), np.uint32); ninl = np.zeros(max(n_pairs, 1), np.uint32); nr = np.zeros(max(n_pairs, 1), np.uint32)
+    rinl = np.zeros(max(nm, 1), np.uint32); E = np.zeros((max(n_pairs, 1), 9)); st = np.zeros((max(n_pairs, 1), 2))
+    p = lambda a: a.ctypes.data_as(_vp)   # noqa: E731
+    check(lib().omvg_geom_angular_acransac(int(device), ESSENTIAL_UPRIGHT if upright else ESSENTIAL_ANGULAR, ctypes.c_uint64(n_pairs), p(off),
+                                           p(bI), p(bJ), ctypes.c_double(precision_deg), ctypes.c_uint32(max_iterations),
+                                           p(inl), p(ninl), p(E), p(st), p(nr), p(rinl)))
+    out = []
+    for q in range(n_pairs):
+        a = int(off[q])
+        out.append(dict(inliers=inl[a:a + int(ninl[q])].copy(), ransac_inliers=rinl[a:a + int(nr[q])].copy(), F=E[q].reshape(3, 3).copy(),
+                        error_max=float(st[q, 0]), min_nfa=float(st[q, 1])))
+    return out
+
+
+def debug_angular_solver(b1, b2, upright: bool = False, device: int = 0):
+    """The device eight-point (or upright three-point) solver on n samples of 8 (3) bearing pairs [n, ms, 3] (validation
+    aid).  -> E [n, 3, 3]"""
+    ms = 3 if upright else 8
+    b1 = np.ascontiguousarray(b1, np.float64).reshape(-1, ms, 3); b2 = np.ascontiguousarray(b2, np.float64).reshape(-1, ms, 3)
+    n = len(b1); assert len(b2) == n
+    E = np.zeros((max(n, 1), 9))
+    p = lambda a: a.ctypes.data_as(_vp)   # noqa: E731
+    check(lib().omvg_geom_debug_angular_solver(int(device), ESSENTIAL_UPRIGHT if upright else ESSENTIAL_ANGULAR, ctypes.c_uint32(n), p(b1), p(b2), p(E)))
+    return E[:n].reshape(n, 3, 3).copy()
+
+
+def debug_relative_pose(E, b1, b2, index, device: int = 0):
+    """RelativePoseFromEssential(b1, b2, E, index) as the device filter runs it (validation aid).
+    -> dict(counts [4] (cheirality count per pose of MotionFromEssential), selected (the chosen pose's list), ok)"""
+    E = np.ascontiguousarray(E, np.float64).reshape(9)
+    b1 = np.ascontiguousarray(b1, np.float64).reshape(-1, 3); b2 = np.ascontiguousarray(b2, np.float64).reshape(-1, 3)
+    idx = np.ascontiguousarray(index, np.uint32).reshape(-1)
+    assert len(b1) == len(b2)
+    counts = np.zeros(4, np.int32); sel = np.zeros(max(len(idx), 1), np.uint32); ns = np.zeros(1, np.uint32); ok = np.zeros(1, np.int32)
+    p = lambda a: a.ctypes.data_as(_vp)   # noqa: E731
+    check(lib().omvg_geom_debug_relative_pose(int(device), p(E), ctypes.c_uint32(len(b1)), p(b1), p(b2), ctypes.c_uint32(len(idx)), p(idx),
+                                              p(counts), p(sel), p(ns), p(ok)))
+    return dict(counts=counts, selected=sel[:int(ns[0])].copy(), ok=bool(ok[0]))

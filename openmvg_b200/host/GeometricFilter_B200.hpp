@@ -12,6 +12,13 @@
 // Robust_model_estimation_E is GeometricFilter_EMatrix_AC (E_ACRobust.hpp:55-150: five-point essential matrix of calibrated
 // views): pairs whose views lack an intrinsic or have a non-pinhole one are skipped and not kept, as the reference skips
 // them; K comes from Pinhole_Intrinsic::K(); the pair is kept iff it has more than 2.5 * 5 inliers.
+// Robust_model_estimation_EAngular / _EUpright are GeometricFilter_ESphericalMatrix_AC_Angular<false / true>
+// (E_ACRobust_Angular.hpp:52-160: eight-point / upright three-point essential matrix on bearing vectors, any camera type,
+// spherical included): pairs whose views lack an intrinsic are skipped and not kept; the bearings are openMVG's own
+// (*cam)(MatchesPairToMat(...)); all pairs go to omvg_geom_angular_acransac in one call (AC-RANSAC, then
+// RelativePoseFromEssential), and a pair is kept iff its list has more than 2.5 * 8 (2.5 * 3) entries.  With
+// b_guided_matching the reference's Geometry_guided_matching of this functor only logs "Not yet implemented" and the
+// pair is inserted with the EMPTY list it leaves (GeometricFilter.hpp:103-116); the shim does the same, logging once.
 //
 // Guided matching (b_guided_matching, openMVG_main_GeometricFilter's -r; GeometricFilter.hpp:96-123): the kept pairs go
 // through geometry_aware::GuidedMatching on the device in ONE omvg_match_guided_run call, and its result replaces the
@@ -63,6 +70,84 @@ struct ImageCollectionGeometricFilter_B200
   bool Robust_model_estimation_E(const matching::PairWiseMatches & putative_matches, double dPrecision = 4.0, uint32_t iteration = 2048,
                                  system::ProgressInterface * my_progress_bar = nullptr, bool b_guided_matching = false, double d_distance_ratio = 0.6)
   { return Robust_model_estimation(OMVG_GEOM_ESSENTIAL, putative_matches, dPrecision, iteration, my_progress_bar, b_guided_matching, d_distance_ratio); }
+
+  // angular E models (GeometricFilter_ESphericalMatrix_AC_Angular<false | true>(dPrecision, iteration)): dPrecision in
+  // degrees; kept iff more than 2.5 * 8 (eight-point) or 2.5 * 3 (upright) entries after the cheirality step
+  bool Robust_model_estimation_EAngular(const matching::PairWiseMatches & putative_matches, double dPrecision = 4.0, uint32_t iteration = 2048,
+                                        system::ProgressInterface * my_progress_bar = nullptr, bool b_guided_matching = false, double d_distance_ratio = 0.6)
+  { return Robust_model_estimation_Angular(false, putative_matches, dPrecision, iteration, my_progress_bar, b_guided_matching); }
+  bool Robust_model_estimation_EUpright(const matching::PairWiseMatches & putative_matches, double dPrecision = 4.0, uint32_t iteration = 2048,
+                                        system::ProgressInterface * my_progress_bar = nullptr, bool b_guided_matching = false, double d_distance_ratio = 0.6)
+  { return Robust_model_estimation_Angular(true, putative_matches, dPrecision, iteration, my_progress_bar, b_guided_matching); }
+
+  bool Robust_model_estimation_Angular(bool upright, const matching::PairWiseMatches & putative_matches, double dPrecision, uint32_t iteration,
+                                       system::ProgressInterface * my_progress_bar = nullptr, bool b_guided_matching = false)
+  {
+    if (!my_progress_bar) my_progress_bar = &system::ProgressInterface::dummy();
+    my_progress_bar->Restart(putative_matches.size(), "- Geometric filtering (B200) -");
+    std::vector<uint64_t> offsets(1, 0);
+    std::vector<double> bI, bJ;
+    std::vector<const std::pair<const Pair, matching::IndMatches> *> order;
+    size_t skipped = 0;
+    for (const auto & it : putative_matches)
+    {
+      const cameras::IntrinsicBase * cam[2] = {nullptr, nullptr};    // E_ACRobust_Angular.hpp:78-99
+      const IndexT ids[2] = {it.first.first, it.first.second};
+      for (int k = 0; k < 2; ++k)
+      {
+        const IndexT id_intrinsic = sfm_data_->views.at(ids[k])->id_intrinsic;
+        if (sfm_data_->GetIntrinsics().count(id_intrinsic)) cam[k] = sfm_data_->GetIntrinsics().at(id_intrinsic).get();
+      }
+      if (!cam[0] || !cam[1])
+      {
+        ++skipped;
+        continue;
+      }
+      Mat2X a, b;
+      MatchesPairToMat(it.first, it.second, sfm_data_, regions_provider_, a, b);
+      const Mat3X ba = (*cam[0])(a), bb = (*cam[1])(b);               // E_ACRobust_Angular.hpp:105-107
+      for (Mat3X::Index k = 0; k < ba.cols(); ++k)
+        for (int c = 0; c < 3; ++c) { bI.push_back(ba(c, k)); bJ.push_back(bb(c, k)); }
+      offsets.push_back(offsets.back() + static_cast<uint64_t>(ba.cols()));
+      order.push_back(&it);
+    }
+    const size_t n_pairs = order.size();
+    std::vector<uint32_t> inliers(bI.size() / 3 + 1);
+    n_inliers_.assign(n_pairs + 1, 0); F_.assign(9 * n_pairs, 0.0); stats_.assign(2 * n_pairs, 0.0);
+    _map_GeometricMatches.clear();
+    const int rc = omvg_geom_angular_acransac(device_, upright ? OMVG_GEOM_ESSENTIAL_UPRIGHT : OMVG_GEOM_ESSENTIAL_ANGULAR, n_pairs, offsets.data(),
+                                              bI.data(), bJ.data(), dPrecision, iteration, inliers.data(), n_inliers_.data(), F_.data(),
+                                              stats_.data(), nullptr, nullptr);
+    for (size_t p = 0; p < skipped; ++p) ++(*my_progress_bar);
+    if (rc != OMVG_OK)
+    {
+      OPENMVG_LOG_ERROR << "omvg_b200: " << omvg_last_error();
+      return false;
+    }
+    const double min_samples = upright ? 3.0 : 8.0;
+    bool logged = false;
+    for (size_t p = 0; p < n_pairs; ++p)
+    {
+      if (n_inliers_[p] > min_samples * 2.5)                       // E_ACRobust_Angular.hpp:146
+      {
+        matching::IndMatches geometric_inliers;
+        if (b_guided_matching)
+        {
+          if (!logged) OPENMVG_LOG_ERROR << "Not yet implemented";  // the functor's Geometry_guided_matching
+          logged = true;
+        }
+        else
+        {
+          geometric_inliers.reserve(n_inliers_[p]);
+          for (uint32_t k = 0; k < n_inliers_[p]; ++k) geometric_inliers.push_back(order[p]->second[inliers[offsets[p] + k]]);
+        }
+        _map_GeometricMatches.insert({order[p]->first, std::move(geometric_inliers)});
+      }
+      ++(*my_progress_bar);
+    }
+    n_inliers_.resize(n_pairs);
+    return true;
+  }
 
   bool Robust_model_estimation(int32_t model, const matching::PairWiseMatches & putative_matches, double dPrecision, uint32_t iteration,
                                system::ProgressInterface * my_progress_bar = nullptr, bool b_guided_matching = false, double d_distance_ratio = 0.6)
@@ -247,6 +332,7 @@ struct ImageCollectionGeometricFilter_B200
   int device_;
   matching::PairWiseMatches _map_GeometricMatches;
   std::vector<double> F_, stats_;                               // per pair sent (map order): un-normalised F (H, E), {errorMax, minNFA}
+  std::vector<uint32_t> n_inliers_;                             // angular models, per pair sent: the list length after the cheirality step
 };
 
 }  // namespace matching_image_collection

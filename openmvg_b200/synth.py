@@ -299,6 +299,57 @@ def calibrated_two_view_matches(n: int, outlier_frac: float = 0.3, seed: int = 3
             tuple(float(v) for v in intr_I), tuple(float(v) for v in intr_J))
 
 
+def spherical_bearings(xy: np.ndarray, wh=(2000, 1000)) -> np.ndarray:
+    """Bearing vectors of equirectangular pixel positions [n, 2], as Camera_Spherical::operator() forms them
+    (cameras/Camera_Spherical.hpp:115-131), with numpy's sin / cos."""
+    w, h = wh
+    size = float(max(w, h))
+    lon = (xy[:, 0] - w / 2.0) / size * 2 * np.pi
+    lat = -((xy[:, 1] - h / 2.0) / size) * 2 * np.pi
+    return np.stack([np.cos(lat) * np.sin(lon), -np.sin(lat), np.cos(lat) * np.cos(lon)], 1)
+
+
+ANGULAR_MOTIONS = ("general", "short", "forward", "full", "upright", "upright_tilt", "rotation")
+
+
+def spherical_two_view_matches(n: int, outlier_frac: float = 0.3, seed: int = 3, motion: str = "general", wh=(2000, 1000),
+                               noise_px: float = 0.3):
+    """Putative matches of one pair of 360° (equirectangular) views for the angular essential-matrix filters (DESIGN
+    §3.10).  motion: "general" (sideways + rotation), "short" (a baseline of 1 % of the depth), "forward" (along the
+    optical axis), "full" (general motion, points all around the camera, half of them behind it: bearing z < 0),
+    "upright" (a rotation about y and a translation with t_y = 0, the upright solver's model), "upright_tilt" (the same
+    with a small t_y and a small tilt, off that model), "rotation" (a baseline of 1e-6 of the depth: the cheirality test
+    is ambiguous).  Pixel positions are rounded to float32, as openMVG stores features, and the bearings are formed
+    from them.  -> (xy_I [n,2], xy_J [n,2], bI [n,3], bJ [n,3], inlier mask [n])"""
+    rng = np.random.default_rng(seed)
+    w, h = wh
+    if motion == "full":
+        d = rng.normal(size=(n, 3))
+    else:
+        d = np.stack([rng.uniform(-1.2, 1.2, n), rng.uniform(-0.8, 0.8, n), np.ones(n)], 1)
+    X = d / np.linalg.norm(d, axis=1, keepdims=True) * rng.uniform(3.0, 10.0, (n, 1))
+    R2, C2 = {"general": (_rodrigues(np.array([0.03, -0.25, 0.02])), np.array([1.2, 0.05, 0.3])),
+              "short": (_rodrigues(np.array([0.01, -0.02, 0.005])), np.array([0.06, 0.01, 0.02])),
+              "forward": (_rodrigues(np.array([0.01, 0.02, -0.01])), np.array([0.02, -0.01, 1.5])),
+              "full": (_rodrigues(np.array([0.2, 0.9, -0.1])), np.array([0.9, -0.3, -0.6])),
+              "upright": (_rodrigues(np.array([0.0, 0.35, 0.0])), np.array([0.8, 0.0, 0.5])),
+              "upright_tilt": (_rodrigues(np.array([0.02, 0.35, -0.015])), np.array([0.8, 0.04, 0.5])),
+              "rotation": (_rodrigues(np.array([0.05, 0.3, -0.02])), np.array([1e-6, 0.0, 0.0]))}[motion]
+
+    def pix(b):
+        b = b / np.linalg.norm(b, axis=1, keepdims=True)
+        lon = np.arctan2(b[:, 0], b[:, 2]); lat = -np.arcsin(np.clip(b[:, 1], -1, 1))
+        size = float(max(w, h))
+        return np.stack([lon / (2 * np.pi) * size + w / 2.0, -lat / (2 * np.pi) * size + h / 2.0], 1)
+    xI = pix(X) + rng.normal(0, noise_px, (n, 2))
+    xJ = pix((X - C2) @ R2.T) + rng.normal(0, noise_px, (n, 2))
+    out = rng.random(n) < outlier_frac
+    xJ[out] = np.stack([rng.uniform(0, w, int(out.sum())), rng.uniform(0, h, int(out.sum()))], 1)
+    xI = np.mod(xI, [w, h]).astype(np.float32).astype(np.float64)
+    xJ = np.mod(xJ, [w, h]).astype(np.float32).astype(np.float64)
+    return xI, xJ, spherical_bearings(xI, wh), spherical_bearings(xJ, wh), ~out
+
+
 def guided_scene(n_views: int, n_feat, seed: int = 9, wh=(1600, 1200), planar: bool = False, shared_frac: float = 0.6,
                  n_dup: int = 0, desc_noise: int = 8, noise_px: float = 0.5):
     """Per-view feature positions and SIFT-like descriptors of one 3-D scene for guided matching (DESIGN §3.9).
